@@ -37,6 +37,7 @@ void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
 cudaError_t upload_model(const trl::ModelConst& mc);
+cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_cg
 
@@ -208,28 +209,54 @@ static int fill_model(trl_handle* h, uint64_t rng_seed) {
     if (m.max_depth >= 16) return fail("kinematic tree too deep for the 4-round ancestor jumps");
     if (m.nj > 31) return fail("lane 31 must stay idle (zero source of the warp passes)");
     {
-        // inward-pass schedule (parents precede children in index order, so walk the links backwards)
-        std::vector<int> earliest(m.nj, 0);
-        for (int j = 0; j < m.nj; ++j) { m.acc_round[j] = -1; m.acc_src[j] = ~0ull; }
-        for (int p = m.nj - 1; p >= 0; --p) {
-            // children of p, by the earliest round they can be eliminated in
+        // chain schedule.  Summation order at a branch point: children by the earliest step their subtree is complete in (ties by
+        // index) -- the order of the level-synchronous schedule this one replaced, so the sums are the same to the bit
+        std::vector<int> earliest(m.nj, 0), nch(m.nj, 0);
+        std::vector<std::vector<int>> merge_order(m.nj);
+        for (int j = 1; j < m.nj; ++j) ++nch[m.parent[j]];
+        for (int p = m.nj - 1; p >= 0; --p) {     // parents precede children in index order
             std::vector<std::pair<int, int>> ch;
             for (int c = 0; c < 4; ++c) if (m.child[p][c] >= 0) ch.push_back({earliest[m.child[p][c]], m.child[p][c]});
             std::sort(ch.begin(), ch.end());
             int last = -1;
-            for (auto& ec : ch) {
-                int t = std::max(ec.first, last + 1);
-                m.acc_round[ec.second] = t;
-                last = t;
-            }
+            for (auto& ec : ch) { merge_order[p].push_back(ec.second); last = std::max(ec.first, last + 1); }
             earliest[p] = last + 1;
         }
-        m.acc_rounds = earliest[0];
-        m.acc_round[0] = m.acc_rounds;     // the root is never eliminated
-        if (m.acc_rounds > 12) return fail("inward-pass schedule longer than 12 rounds");
-        for (int j = 1; j < m.nj; ++j) {
-            const int p = m.parent[j], r = m.acc_round[j];
-            m.acc_src[p] = (m.acc_src[p] & ~(31ull << (5 * r))) | ((unsigned long long)j << (5 * r));
+        // chain tops: the root and every child of a link with more than one child; chain 0 is the root's
+        std::vector<int> tops, chain_of(m.nj, -1);
+        for (int j = 0; j < m.nj; ++j) if (j == 0 || nch[m.parent[j]] != 1) tops.push_back(j);
+        m.n_chains = (int)tops.size();
+        if (m.n_chains > kWarp) return fail("more chains than lanes");
+        std::vector<int> bottom(m.n_chains);
+        for (int c = 0; c < m.n_chains; ++c) {
+            std::vector<int> links{tops[c]};
+            while (nch[links.back()] == 1) links.push_back(m.child[links.back()][0]);
+            if ((int)links.size() > 12) return fail("kinematic chain longer than 12 links");
+            m.chain_len[c] = (int)links.size();
+            m.chain_links[c] = 0;
+            for (int i = 0; i < m.chain_len[c]; ++i) {
+                m.chain_links[c] |= (unsigned long long)links[m.chain_len[c] - 1 - i] << (5 * i);
+                chain_of[links[i]] = c;
+            }
+            bottom[c] = links.back();
+            m.chain_up[c] = tops[c] == 0 ? -1 : m.parent[tops[c]];
+        }
+        m.chain_levels = 0;
+        for (int c = m.n_chains - 1; c >= 0; --c) {    // a child chain's top has a larger index than its parent chain's bottom
+            m.chain_merge[c] = 0;
+            int lev = 0;
+            for (int q = 0; q < 4; ++q) {
+                const int ch = (nch[bottom[c]] > 1 && q < nch[bottom[c]]) ? merge_order[bottom[c]][q] : -1;
+                const int cc = ch >= 0 ? chain_of[ch] : 31;
+                if (ch >= 0) lev = std::max(lev, m.chain_level[cc] + 1);
+                m.chain_merge[c] |= cc << (5 * q);
+            }
+            m.chain_level[c] = lev;
+            m.chain_levels = std::max(m.chain_levels, lev + 1);
+        }
+        for (int l = 0; l < m.chain_levels; ++l) {
+            m.chain_level_len[l] = 0;
+            for (int c = 0; c < m.n_chains; ++c) if (m.chain_level[c] == l) m.chain_level_len[l] = std::max(m.chain_level_len[l], m.chain_len[c]);
         }
     }
     for (int j = 0; j < m.nj; ++j) {
@@ -639,7 +666,7 @@ static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mo
     };
     g_model_owner = nullptr;
     if (ensure_model(h)) return bail("upload_model failed");
-    if (!ck(configure_step_kernels(), "configure_step_kernels")) return bail("");
+    if (!ck(configure_step_kernels(), "configure_step_kernels") || !ck(trl_cg::configure_step_kernels(), "configure_step_kernels")) return bail("");
     if (!ck(configure_decide_kernel(), "configure_decide_kernel")) return bail("");
     if (!ck(configure_decide2_kernels(), "configure_decide2_kernels")) return bail("");
     {

@@ -13,6 +13,9 @@
 #include "../../include/terrainrl_b200.h"
 #include "trl_handle.h"
 
+namespace trl { cudaError_t step_phase_clocks(unsigned long long* out, int reset); }
+namespace trl_cg { cudaError_t step_phase_clocks(unsigned long long* out, int reset); }
+
 namespace trl_probe {
 using namespace trl;
 
@@ -118,5 +121,18 @@ extern "C" int trl_get_layer_state(trl_handle* h, int env, const char* layer_nam
     const int n = std::min(hit->size, cap);
     if (cudaMemcpy(out, h->probe_dump + hit->off, (size_t)n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return trl_fail("trl_get_layer_state: copy failed");
     if (n_out) *n_out = hit->size;
+    return 0;
+}
+
+// Per-phase clock64() sums of the env-step kernel (both builds: main and catch-up launches), in a TRL_PHASE_CLOCKS=1 build only.
+// out[0..n-2] = cycles summed over warps per phase, out[n-1] = env-steps (physics halves) counted; reset zeroes the counters.
+extern "C" int trl_debug_step_phases(trl_handle* h, unsigned long long* out, int n, int reset) {
+    constexpr int kSlots = 10;
+    if (!h || !out || n != kSlots) return trl_fail("trl_debug_step_phases: null handle / output, or n != 10");
+    if (cudaStreamSynchronize(h->stream) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return trl_fail("trl_debug_step_phases: sync failed");
+    unsigned long long a[kSlots], b[kSlots];
+    if (trl::step_phase_clocks(a, reset) != cudaSuccess || trl_cg::step_phase_clocks(b, reset) != cudaSuccess)
+        return trl_fail("trl_debug_step_phases: the library was built without -DTRL_PHASE_CLOCKS=1 (TRL_VARIANT=phase_clocks)");
+    for (int k = 0; k < kSlots; ++k) out[k] = a[k] + b[k];
     return 0;
 }

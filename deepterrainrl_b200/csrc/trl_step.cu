@@ -1,9 +1,10 @@
 // deepterrainrl_b200 -- the env-step kernel (sm_90a), warp-per-environment formulation.
 //
-// One environment per WARP: lane j owns link j of the kinematic tree (21 links) and, for the dense solve, row j of
-// the 23x23 system; every tree recursion is level-synchronous over the tree depth (9 for the dog) with the
-// parent <-> child hand-off done by warp shuffles, so per-link quantities live in registers and shared memory only
-// holds the mass matrix.  All spatial quantities are planar 3-vectors expressed in WORLD axes about the root joint's
+// One environment per WARP: lane j owns link j of the kinematic tree (21 links) for the kinematics, contacts and integration.
+// The tree recursions (composite sums, articulated-body eliminations, outward accelerations) run one lane per CHAIN -- a maximal run
+// of single-child links -- through a per-warp, link-indexed block in shared memory: a chain lane eliminates its links one after the
+// other in registers, and chains meet only at branch points, one warp barrier per level of the chain tree.  All spatial
+// quantities are planar 3-vectors expressed in WORLD axes about the root joint's
 // current position O (an inertial frame that instantaneously coincides with the root), which removes every
 // per-link coordinate transform from the recursions: motion (w, vOx, vOy), force (nO, fx, fy), joint axis of a
 // revolute joint at r (relative to O): S = (1, r_y, -r_x).
@@ -11,8 +12,8 @@
 // One launch = the *controller half* of env-step k followed by the *physics half* of env-step k+1:
 //
 //   ctrl half  (reference: cSimCharacter::Update -> cDogController::Update, sim/DogController.cpp:229-268)
-//     CRBA mass matrix + RNEA bias force with the reference's Cj (restates sim/RBDUtil.cpp:4-176 in planar algebra)
-//     ApplyFeedback, stable-PD solve (register-resident LDL^T, one row per lane), gravity compensation,
+//     RNEA bias force with the reference's Cj and composite inertias (restates sim/RBDUtil.cpp:4-176 in planar algebra)
+//     ApplyFeedback, stable-PD solve (M + h Kd) acc = rhs by the articulated-body recursion (h Kd as joint armature), gravity compensation,
 //     virtual forces, torque clamp (sim/Joint.cpp:257-264), fall counters (sim/SimCharSoftFall.cpp:74-125),
 //     cycle bookkeeping: reward, tuple record, episode statistics (scenarios/ScenarioExp.cpp:209-243)
 //   [end of outer update: fall -> episode reset, scenarios/ScenarioPoliEval.cpp:110-125, ScenarioExp.cpp:83-98]
@@ -26,6 +27,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "trl_terrain.cuh"
 #include "trl_types.h"
@@ -80,57 +82,56 @@ constexpr int kStepSkipPending = 8, kStepCatchUp = 16;   // flag bits of trl_ste
 // of env-steps a catch-up launch advances its envs by
 constexpr double kClearMargin = 0.05;   // >= contact_tol * sqrt(1 + slope^2) for any slope the generators produce
 constexpr int kZeroLane = 31;   // always idle (nj <= 23): its per-link registers are zero, used as the "no source" lane
-constexpr int kTri = kMaxDof * (kMaxDof + 1) / 2;   // 276
-// per-warp shared scratch (doubles)
-constexpr int X_M = 0;
+// per-warp shared scratch (doubles; every block starts 16-byte aligned)
+// Link block: one slot per link, written by the link lanes and walked by the chain lanes (chain_inward / chain_outward).  A slot is
+// 9 double2, an odd number of 16-byte units, so the 128-bit accesses of 8 lanes to 8 different links fall in distinct banks.
+constexpr int kLinkStride = 18;
+enum {
+    LK_IA = 0,     // [0, 9): articulated inertia (a, bx, by, cxx, cxy, cyy) + bias force (n, fx, fy) of the link alone; composite sums
+    LK_TAU = 9,    // joint force of the elimination
+    LK_CV = 10,    // (cvx, cvy): velocity-product acceleration c_j
+    LK_S = 12,     // (s1, s2): joint axis S_j = (1, s1, s2)
+    LK_LIM = 14,   // (lim_f, cl): implicit joint term, u_j -= lim_f, D_j += dt * cl
+    // written by the elimination over [0, 5) and by the outward pass
+    LK_U = 0, LK_DINV = 3, LK_UU = 4, LK_QDD = 5, LK_ACC = 6 /* (aw, ax, ay) */
+};
+constexpr int kChainStride = 10;                            // per chain: the 9 values its top link hands to its parent link
+constexpr int X_LNK = 0;
+constexpr int X_CHO = X_LNK + kMaxJoints * kLinkStride;
+constexpr int X_CHO_END = X_CHO + kMaxJoints * kChainStride;
 // Experiments (shuffles are a large share of the kernel's instructions).  Each knob moves one
 // family of lane-to-lane exchanges from warp shuffles (2 SHFL + register moves per double) to per-warp shared memory (128-bit
 // stores / loads); values and operation order are untouched, so every variant is bit-identical to the default build
-// (tests/test_simt_cpu.py checks that on the CPU emulator).  Default build: the LDL^T exchange on, the others off.  -DTRL_SMEM_XCHG=1: all on.
+// (tests/test_simt_cpu.py checks that on the CPU emulator).  Default build: all off.  -DTRL_SMEM_XCHG=1: all on.
+// TRL_ACCUM_SMEM and TRL_LDLT_SMEM name exchanges the chain passes removed (the round-by-round child -> parent hand-off, the
+// LDL^T pivot column); they are accepted and change nothing.
 #ifndef TRL_SMEM_XCHG
 #define TRL_SMEM_XCHG 0
-#endif
-#ifndef TRL_ACCUM_SMEM
-#define TRL_ACCUM_SMEM TRL_SMEM_XCHG     // child -> parent hand-off of the inward rounds (9 doubles x 9 rounds x 5 sub-steps)
-#endif
-#ifndef TRL_LDLT_SMEM
-#define TRL_LDLT_SMEM 1                  // ON by default since round 2 (fewer spill stores than the shuffle exchange).  pivot column of the register LDL^T + fused forward substitution (253 + 23 doubles)
 #endif
 #ifndef TRL_KIN_SMEM
 #define TRL_KIN_SMEM TRL_SMEM_XCHG       // pointer-jumping prefix sums of the kinematics (26 doubles x 6 per env-step)
 #endif
 #ifndef TRL_OUTWARD_SMEM
-#define TRL_OUTWARD_SMEM TRL_SMEM_XCHG   // parent -> child accelerations of the outward pass + floating-base broadcast (36 doubles x 5)
+#define TRL_OUTWARD_SMEM TRL_SMEM_XCHG   // floating-base broadcast of the root's articulated inertia (9 doubles x 6 per env-step)
 #endif
 #ifndef TRL_CONTACT_SMEM
 #define TRL_CONTACT_SMEM TRL_SMEM_XCHG   // corner lanes read their body's kinematics, owners collect contact forces (7-21 + 9 per contact, x 5)
 #endif
-#define TRL_SMEM_ALIGNED (TRL_ACCUM_SMEM || TRL_LDLT_SMEM || TRL_KIN_SMEM || TRL_OUTWARD_SMEM || TRL_CONTACT_SMEM)
-constexpr int X_M_END = X_M + kTri + 4;
-#if TRL_ACCUM_SMEM || TRL_CONTACT_SMEM
+#if TRL_CONTACT_SMEM
 constexpr int kAccStride = 10;                              // doubles per lane slot: 9 values, padded to 80 B (128-bit accesses stay conflict-free)
-constexpr int X_ACC = (X_M_END + 1) & ~1;                   // 16-byte aligned
+constexpr int X_ACC = X_CHO_END;
 constexpr int X_ACC_END = X_ACC + kWarp * kAccStride;
 #else
-constexpr int X_ACC_END = X_M_END;
-#endif
-#if TRL_LDLT_SMEM
-constexpr int kColStride = kWarp + 2;                       // 32 column entries + the solved right-hand-side entry, even (16-byte rows)
-constexpr int X_COL = (X_ACC_END + 1) & ~1;                 // two buffers: step j writes buffer j & 1
-constexpr int X_COL_END = X_COL + 2 * kColStride;
-#else
-constexpr int X_COL_END = X_ACC_END;
+constexpr int X_ACC_END = X_CHO_END;
 #endif
 #if TRL_KIN_SMEM
-constexpr int X_PFX = (X_COL_END + 1) & ~1;                 // three buffers of 32 double2: prefix rounds alternate 0 / 1, buffer 2 = (cos, sin) exchange
+constexpr int X_PFX = (X_ACC_END + 1) & ~1;                 // three buffers of 32 double2: prefix rounds alternate 0 / 1, buffer 2 = (cos, sin) exchange
 constexpr int X_PFX_END = X_PFX + 3 * 2 * kWarp;
 #else
-constexpr int X_PFX_END = X_COL_END;
+constexpr int X_PFX_END = X_ACC_END;
 #endif
 #if TRL_OUTWARD_SMEM
-constexpr int kOutBuf = 3 * kWarp;                          // (aw, ax) as double2 [32] + ay [32]
-constexpr int X_OUT = (X_PFX_END + 1) & ~1;                 // two buffers (level parity) + the 9 floating-base values of lane 0
-constexpr int X_BASE = X_OUT + 2 * kOutBuf;
+constexpr int X_BASE = (X_PFX_END + 1) & ~1;                // the 9 floating-base values of lane 0
 constexpr int X_OUT_END = X_BASE + 10;
 #else
 constexpr int X_OUT_END = X_PFX_END;
@@ -141,7 +142,33 @@ constexpr int X_KIN_END = X_KIN + 7 * kWarp;
 #else
 constexpr int X_KIN_END = X_OUT_END;
 #endif
-constexpr int X_END = TRL_SMEM_ALIGNED ? ((X_KIN_END + 1) & ~1) : X_KIN_END;
+constexpr int X_END = (X_KIN_END + 1) & ~1;
+// Measurement build (-DTRL_PHASE_CLOCKS=1, TRL_VARIANT=phase_clocks): lane 0 of every warp adds the clock64() delta of each
+// phase of the launch to g_phase_clocks[phase]; slot kNumPhases counts the physics halves (env-steps).  Read out by
+// trl_debug_step_phases (trl_probe.cu), printed by tools/step_phase_probe.py.  The product build compiles none of it.
+#ifndef TRL_PHASE_CLOCKS
+#define TRL_PHASE_CLOCKS 0
+#endif
+enum StepPhase { PH_LOAD, PH_RNEA, PH_SOLVE, PH_CTRL_REST, PH_KIN, PH_CONTACT, PH_INWARD, PH_OUTWARD, PH_TAIL, kNumPhases };
+#if TRL_PHASE_CLOCKS
+__device__ unsigned long long g_phase_clocks[kNumPhases + 1];
+#define TRL_CLK_DECL(a, b) , int a, int b      // phases a helper's parts are counted under
+#define TRL_CLK_ARG(a, b) , a, b
+#define TRL_CLK_BEGIN(t) long long t = clock64()
+#define TRL_CLK_RESET(t) (t) = clock64()
+#define TRL_CLK_END(p, t)                                                                                              \
+    do {                                                                                                               \
+        const long long n_ = clock64();                                                                                \
+        if ((threadIdx.x & 31) == 0) atomicAdd(&g_phase_clocks[(p)], (unsigned long long)(n_ - (t)));                  \
+        (t) = n_;                                                                                                      \
+    } while (0)
+#else
+#define TRL_CLK_DECL(a, b)
+#define TRL_CLK_ARG(a, b)
+#define TRL_CLK_BEGIN(t)
+#define TRL_CLK_RESET(t)
+#define TRL_CLK_END(p, t)
+#endif
 // the scratch pointer is only threaded through the helpers that need it, so the default build's code is untouched
 #if TRL_KIN_SMEM
 #define TRL_KIN_XS_DECL , double* xs, int lane
@@ -161,13 +188,6 @@ constexpr int X_END = TRL_SMEM_ALIGNED ? ((X_KIN_END + 1) & ~1) : X_KIN_END;
 #define TRL_REUSE_KIN_DECL , const Kin* k0
 #else
 #define TRL_REUSE_KIN_DECL
-#endif
-#if TRL_SMEM_ALIGNED
-#define TRL_PHYS_XS_DECL , double* xs
-#define TRL_PHYS_XS_ARG , xs
-#else
-#define TRL_PHYS_XS_DECL
-#define TRL_PHYS_XS_ARG
 #endif
 
 // 128-bit shared-memory accesses of the experiment builds need 16-byte aligned addresses (a misaligned one faults on the GPU);
@@ -418,7 +438,7 @@ __device__ void store_rng(Lane& L, const CounterRng& r) {
 #endif
 #if TRL_LINK_SMEM
 enum { LF_AX, LF_AY, LF_MASS, LF_BAX, LF_BAY, LF_IZZ, LF_LIM_LO, LF_LIM_HI, LF_NUM };
-enum { LI_PARENT, LI_DEPTH, LI_ACC_ROUND, LI_ANC1, LI_ANC2, LI_ANC4, LI_ANC8, LI_NUM };
+enum { LI_PARENT, LI_DEPTH, LI_ANC1, LI_ANC2, LI_ANC4, LI_ANC8, LI_CH_LEN, LI_CH_LEVEL, LI_CH_MERGE, LI_CH_UP, LI_NUM };
 // a field of the table as a value: every read is one conflict-free LDS (tables are [field][lane])
 template <int F> struct LkD { const double* p; __device__ __forceinline__ operator double() const { return p[F * kWarp]; } };
 template <int F> struct LkI { const int* p; __device__ __forceinline__ operator int() const { return p[F * kWarp]; } };
@@ -430,8 +450,8 @@ struct LinkTables {
 };
 struct LinkC {
     int act;            // lane < nj
-    LkI<LI_PARENT> parent; LkI<LI_DEPTH> depth; LkI<LI_ACC_ROUND> acc_round;
-    LkU acc_src;
+    LkI<LI_PARENT> parent; LkI<LI_DEPTH> depth;
+    LkU ch_links; LkI<LI_CH_LEN> ch_len; LkI<LI_CH_LEVEL> ch_level; LkI<LI_CH_MERGE> ch_merge; LkI<LI_CH_UP> ch_up;
     LkI<LI_ANC1> anc1; LkI<LI_ANC2> anc2; LkI<LI_ANC4> anc4; LkI<LI_ANC8> anc8;
     LkD<LF_AX> ax; LkD<LF_AY> ay;
     LkD<LF_MASS> mass; LkD<LF_BAX> bax; LkD<LF_BAY> bay; LkD<LF_IZZ> izz_c;
@@ -443,8 +463,8 @@ struct LinkTables;
 struct LinkC {
     int act;            // lane < nj
     int parent, depth;
-    int acc_round;                // inward-pass round in which this link is eliminated (-1 idle lane, acc_rounds root)
-    unsigned long long acc_src;   // 5 bits per inward round: lane to receive from (31 = none)
+    unsigned long long ch_links;  // chain `lane` of the schedule (ModelConst::chain_*; level -1: no chain)
+    int ch_len, ch_level, ch_merge, ch_up;
     int anc1, anc2, anc4, anc8;   // 2^k-th ancestors (31 = none: the idle zero lane) for the pointer-jumping prefix sums
     double ax, ay;      // attach point in the parent's joint frame
     double mass, bax, bay, izz_c;
@@ -464,8 +484,8 @@ struct EnvRegs {
 
 // the link constants of lane `lane` as plain values (constant memory -> registers)
 struct LinkVals {
-    int act, parent, depth, acc_round, anc1, anc2, anc4, anc8;
-    unsigned long long acc_src;
+    int act, parent, depth, anc1, anc2, anc4, anc8, ch_len, ch_level, ch_merge, ch_up;
+    unsigned long long ch_links;
     double ax, ay, mass, bax, bay, izz_c, lim_lo, lim_hi;
 };
 __device__ __forceinline__ LinkVals link_values(int lane) {
@@ -475,8 +495,13 @@ __device__ __forceinline__ LinkVals link_values(int lane) {
     int j = c.act ? lane : 0;
     c.parent = (c.act && j > 0) ? LT(parent, j) : 0;
     c.depth = c.act ? LT(depth, j) : -1;
-    c.acc_round = c.act ? LT(acc_round, j) : -1;
-    c.acc_src = c.act ? LT(acc_src, j) : ~0ull;
+    const bool has_chain = lane < m.n_chains;
+    const int ci = has_chain ? lane : 0;
+    c.ch_links = has_chain ? LT(chain_links, ci) : 0ull;
+    c.ch_len = has_chain ? LT(chain_len, ci) : 0;
+    c.ch_level = has_chain ? LT(chain_level, ci) : -1;
+    c.ch_merge = has_chain ? LT(chain_merge, ci) : ~0;
+    c.ch_up = has_chain ? LT(chain_up, ci) : -1;
     c.anc1 = c.act ? LT2(anc_pow, j, 0) : -1; c.anc2 = c.act ? LT2(anc_pow, j, 1) : -1;
     c.anc4 = c.act ? LT2(anc_pow, j, 2) : -1; c.anc8 = c.act ? LT2(anc_pow, j, 3) : -1;
     if (c.anc1 < 0) c.anc1 = kZeroLane;
@@ -501,8 +526,10 @@ __device__ __forceinline__ void stage_link_tables(LinkTables* t) {
         t->d[LF_AX * kWarp + lane] = v.ax; t->d[LF_AY * kWarp + lane] = v.ay; t->d[LF_MASS * kWarp + lane] = v.mass;
         t->d[LF_BAX * kWarp + lane] = v.bax; t->d[LF_BAY * kWarp + lane] = v.bay; t->d[LF_IZZ * kWarp + lane] = v.izz_c;
         t->d[LF_LIM_LO * kWarp + lane] = v.lim_lo; t->d[LF_LIM_HI * kWarp + lane] = v.lim_hi;
-        t->u[lane] = v.acc_src;
-        t->i[LI_PARENT * kWarp + lane] = v.parent; t->i[LI_DEPTH * kWarp + lane] = v.depth; t->i[LI_ACC_ROUND * kWarp + lane] = v.acc_round;
+        t->u[lane] = v.ch_links;
+        t->i[LI_PARENT * kWarp + lane] = v.parent; t->i[LI_DEPTH * kWarp + lane] = v.depth;
+        t->i[LI_CH_LEN * kWarp + lane] = v.ch_len; t->i[LI_CH_LEVEL * kWarp + lane] = v.ch_level;
+        t->i[LI_CH_MERGE * kWarp + lane] = v.ch_merge; t->i[LI_CH_UP * kWarp + lane] = v.ch_up;
         t->i[LI_ANC1 * kWarp + lane] = v.anc1; t->i[LI_ANC2 * kWarp + lane] = v.anc2; t->i[LI_ANC4 * kWarp + lane] = v.anc4;
         t->i[LI_ANC8 * kWarp + lane] = v.anc8;
     }
@@ -516,13 +543,15 @@ __device__ __forceinline__ LinkC load_link(int lane, const LinkTables* t) {
     c.act = lane < c_model.nj;
     const double* d = t->d + lane;
     const int* i = t->i + lane;
-    c.parent.p = i; c.depth.p = i; c.acc_round.p = i; c.anc1.p = i; c.anc2.p = i; c.anc4.p = i; c.anc8.p = i;
-    c.acc_src.p = t->u + lane;
+    c.parent.p = i; c.depth.p = i; c.anc1.p = i; c.anc2.p = i; c.anc4.p = i; c.anc8.p = i;
+    c.ch_len.p = i; c.ch_level.p = i; c.ch_merge.p = i; c.ch_up.p = i;
+    c.ch_links.p = t->u + lane;
     c.ax.p = d; c.ay.p = d; c.mass.p = d; c.bax.p = d; c.bay.p = d; c.izz_c.p = d; c.lim_lo.p = d; c.lim_hi.p = d;
 #else
     (void)t;
     const LinkVals v = link_values(lane);
-    c.act = v.act; c.parent = v.parent; c.depth = v.depth; c.acc_round = v.acc_round; c.acc_src = v.acc_src;
+    c.act = v.act; c.parent = v.parent; c.depth = v.depth;
+    c.ch_links = v.ch_links; c.ch_len = v.ch_len; c.ch_level = v.ch_level; c.ch_merge = v.ch_merge; c.ch_up = v.ch_up;
     c.anc1 = v.anc1; c.anc2 = v.anc2; c.anc4 = v.anc4; c.anc8 = v.anc8;
     c.ax = v.ax; c.ay = v.ay; c.mass = v.mass; c.bax = v.bax; c.bay = v.bay; c.izz_c = v.izz_c; c.lim_lo = v.lim_lo; c.lim_hi = v.lim_hi;
 #endif
@@ -595,35 +624,162 @@ __device__ __forceinline__ Kin kinematics(const LinkC& c, const EnvRegs& e TRL_K
     return k;
 }
 
-// child -> parent hand-off at the end of inward round r: every lane adds the NV register values of the one lane its
-// schedule names for this round (lane 31 = none; it is idle and its values are zero, so the add is unconditional)
-#if TRL_ACCUM_SMEM
-// Experiment: the same hand-off staged through shared memory -- every lane stores its
-// NV values as 128-bit words into its slot, the receiver loads the slot of its source lane.  Same values, same additions, so
-// the results are bit-identical to the shuffle form; ~10 memory instructions per round instead of ~4 per value.
-// `xs` (the warp's shared-memory block) must be in scope.
-#define TRL_ACCUM_ROUND(r, NV, vals)                                                        \
-    do {                                                                                    \
-        const int src_ = (int)(acc_src_v >> (5 * (r))) & 31;                                \
-        double2* mine_ = trl_as2<double2>(xs + X_ACC + lane * kAccStride);        \
-        _Pragma("unroll") for (int v_ = 0; v_ + 1 < (NV); v_ += 2) mine_[v_ / 2] = make_double2((vals)[v_], (vals)[v_ + 1]); \
-        if ((NV) & 1) xs[X_ACC + lane * kAccStride + (NV) - 1] = (vals)[(NV) - 1];         \
-        __syncwarp();                                                                       \
-        const double2* from_ = trl_as2<const double2>(xs + X_ACC + src_ * kAccStride); \
-        _Pragma("unroll") for (int v_ = 0; v_ + 1 < (NV); v_ += 2) {                        \
-            const double2 t_ = from_[v_ / 2];                                               \
-            (vals)[v_] += t_.x; (vals)[v_ + 1] += t_.y;                                     \
-        }                                                                                   \
-        if ((NV) & 1) (vals)[(NV) - 1] += xs[X_ACC + src_ * kAccStride + (NV) - 1];         \
-        __syncwarp();                                                                       \
-    } while (0)
+// ================================================================================================ chain passes
+// The tree recursions run one lane per chain (ModelConst::chain_*): the link lanes fill their slots of the link block, then lane c
+// walks chain c through it, carrying the running values in registers from link to link -- in world axes the hand-off to the
+// parent is a plain addition -- and other chains' results are added only at branch points, in the schedule's fixed order.
+// Per-link values live in the link block, never in dynamically indexed register arrays (those would be local memory).
+struct ChainC {
+    unsigned long long links;   // 5 bits per link, bottom first
+    int len, level, merge, up;  // level -1: this lane walks no chain
+};
+__device__ __forceinline__ ChainC chain_of(const LinkC& lc) {
+    return ChainC{lc.ch_links, lc.ch_len, lc.ch_level, lc.ch_merge, lc.ch_up};
+}
+template <int NV>
+__device__ __forceinline__ void load_vals(const double* p, double (&v)[NV]) {
+#pragma unroll
+    for (int k = 0; k + 1 < NV; k += 2) { const double2 t = *trl_as2<const double2>(p + k); v[k] = t.x; v[k + 1] = t.y; }
+    if (NV & 1) v[NV - 1] = p[NV - 1];
+}
+template <int NV>
+__device__ __forceinline__ void store_vals(double* p, const double (&v)[NV]) {
+#pragma unroll
+    for (int k = 0; k + 1 < NV; k += 2) *trl_as2<double2>(p + k) = make_double2(v[k], v[k + 1]);
+    if (NV & 1) p[NV - 1] = v[NV - 1];
+}
+
+// Inward pass, leaf chains first.  Every link's slot value is summed with what its child hands up (own + child; at a branch point
+// own + the child chains in merge order).  kElim: articulated-body elimination of every link but the root -- U_j, 1/D_j and u_j go
+// back to the slot, the reduced inertia and bias force go up; the root's chain lane (lane 0) ends with the root's articulated
+// inertia and bias force in `a`.  !kElim: plain subtree sums (composite inertias), written back to every slot.
+template <int NV, bool kElim>
+__device__ __forceinline__ void chain_inward(double* xs, const ChainC& ch, int lane, double dt, double (&a)[NV]) {
+    const ModelConst& m = c_model;
+#pragma unroll
+    for (int k = 0; k < NV; ++k) a[k] = 0.0;
+    for (int lev = 0; lev < m.chain_levels; ++lev) {
+        const int steps = m.chain_level_len[lev];
+        const bool mine = ch.level == lev;
+        for (int i = 0; i < steps; ++i) {
+            if (!mine || i >= ch.len) continue;
+            const int j = (int)(ch.links >> (5 * i)) & 31;
+            double* sl = xs + X_LNK + j * kLinkStride;
+            double v[NV];
+            load_vals(sl, v);
+            if (i == 0) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int src = (ch.merge >> (5 * q)) & 31;
+                    if (src == 31) continue;
+                    const double* o = xs + X_CHO + src * kChainStride;
+#pragma unroll
+                    for (int k = 0; k < NV; ++k) v[k] += o[k];
+                }
+            } else {
+#pragma unroll
+                for (int k = 0; k < NV; ++k) v[k] += a[k];
+            }
+            if (kElim && j != 0) {
+                const double2 cv = *trl_as2<const double2>(sl + LK_CV), sv = *trl_as2<const double2>(sl + LK_S),
+                              lm = *trl_as2<const double2>(sl + LK_LIM);
+                const double s1 = sv.x, s2 = sv.y;
+                const double U0 = v[0] + v[1] * s1 + v[2] * s2;
+                const double U1 = v[1] + v[3] * s1 + v[4] * s2;
+                const double U2 = v[2] + v[4] * s1 + v[5] * s2;
+                double Dj = U0 + s1 * U1 + s2 * U2;
+                double uu = sl[LK_TAU] - (v[6] + s1 * v[7] + s2 * v[8]);
+                uu -= lm.x;
+                Dj += dt * lm.y;
+                const double dinv = 1.0 / Dj;
+                // Ia = IA - U U^T / D ;  pa = pA + Ia c + U u / D
+                const double n0 = v[0] - U0 * U0 * dinv, n1 = v[1] - U0 * U1 * dinv, n2 = v[2] - U0 * U2 * dinv;
+                const double n3 = v[3] - U1 * U1 * dinv, n4 = v[4] - U1 * U2 * dinv, n5 = v[5] - U2 * U2 * dinv;
+                const double ud = uu * dinv;
+                a[6] = v[6] + (n1 * cv.x + n2 * cv.y + U0 * ud);
+                a[7] = v[7] + (n3 * cv.x + n4 * cv.y + U1 * ud);
+                a[8] = v[8] + (n4 * cv.x + n5 * cv.y + U2 * ud);
+                a[0] = n0; a[1] = n1; a[2] = n2; a[3] = n3; a[4] = n4; a[5] = n5;
+                *trl_as2<double2>(sl + LK_U) = make_double2(U0, U1);
+                *trl_as2<double2>(sl + LK_U + 2) = make_double2(U2, dinv);
+                sl[LK_UU] = uu;
+            } else {
+#pragma unroll
+                for (int k = 0; k < NV; ++k) a[k] = v[k];
+                if (!kElim) store_vals(sl, v);
+            }
+        }
+        if (mine) store_vals(xs + X_CHO + lane * kChainStride, a);
+        __syncwarp();
+    }
+}
+
+// Outward pass, root chain first: qdd_j = (u_j - U_j . (a_parent + c_j)) / D_j, a_j = a_parent + c_j + S_j qdd_j; the root's
+// spatial acceleration is (a0, a1, a2).  qdd and a go to every link's slot.
+__device__ __forceinline__ void chain_outward(double* xs, const ChainC& ch, double a0, double a1, double a2) {
+    const ModelConst& m = c_model;
+    for (int lev = m.chain_levels - 1; lev >= 0; --lev) {
+        const int steps = m.chain_level_len[lev];
+        const bool mine = ch.level == lev;
+        double aw = 0.0, alx = 0.0, aly = 0.0;
+        for (int i = 0; i < steps; ++i) {
+            if (!mine || i >= ch.len) continue;
+            const int j = (int)(ch.links >> (5 * (ch.len - 1 - i))) & 31;
+            double* sl = xs + X_LNK + j * kLinkStride;
+            if (j == 0) {
+                aw = a0; alx = a1; aly = a2;
+            } else {
+                double paw = aw, pax = alx, pay = aly;
+                if (i == 0) {
+                    const double* ps = xs + X_LNK + ch.up * kLinkStride;
+                    const double2 t = *trl_as2<const double2>(ps + LK_ACC);
+                    paw = t.x; pax = t.y; pay = ps[LK_ACC + 2];
+                }
+                const double2 u01 = *trl_as2<const double2>(sl + LK_U), u2d = *trl_as2<const double2>(sl + LK_U + 2);
+                const double2 cv = *trl_as2<const double2>(sl + LK_CV), sv = *trl_as2<const double2>(sl + LK_S);
+                const double bx = pax + cv.x, by = pay + cv.y;
+                const double qdd = (sl[LK_UU] - (u01.x * paw + u01.y * bx + u2d.x * by)) * u2d.y;
+                aw = paw + qdd; alx = bx + sv.x * qdd; aly = by + sv.y * qdd;
+                sl[LK_QDD] = qdd;
+            }
+            *trl_as2<double2>(sl + LK_ACC) = make_double2(aw, alx);
+            sl[LK_ACC + 2] = aly;
+        }
+        __syncwarp();
+    }
+}
+
+// Articulated-body forward dynamics of the tree over the link block: inward eliminations, floating base IA_0 a_0 = -pA_0 (symmetric
+// 3x3 LDL^T, every lane computes it from lane 0's values), outward accelerations.  The caller has filled every link's slot and
+// synchronised the warp; afterwards slot LK_QDD holds each joint's acceleration, (a0, a1, a2) the root's.
+__device__ __forceinline__ void chain_aba(double* xs, const ChainC& ch, int lane, double dt, double& a0, double& a1, double& a2
+                                          TRL_CLK_DECL(ph_in, ph_out)) {
+    TRL_CLK_BEGIN(clk);
+    double ia[9];
+    chain_inward<9, true>(xs, ch, lane, dt, ia);
+    TRL_CLK_END(ph_in, clk);
+    {
+#if TRL_OUTWARD_SMEM
+        double* bs = xs + X_BASE;
+        if (lane == 0) store_vals(bs, ia);
+        __syncwarp();
+        double q[9];
+        load_vals(bs, q);
+        const double a = q[0], bx = q[1], by = q[2], cxx = q[3], cxy = q[4], cyy = q[5];
+        const double r0 = -q[6], r1 = -q[7], r2 = -q[8];
 #else
-#define TRL_ACCUM_ROUND(r, NV, vals)                                                        \
-    do {                                                                                    \
-        const int src_ = (int)(acc_src_v >> (5 * (r))) & 31;                                \
-        _Pragma("unroll") for (int v_ = 0; v_ < (NV); ++v_) (vals)[v_] += shf((vals)[v_], src_); \
-    } while (0)
+        const double a = shf(ia[0], 0), bx = shf(ia[1], 0), by = shf(ia[2], 0), cxx = shf(ia[3], 0), cxy = shf(ia[4], 0), cyy = shf(ia[5], 0);
+        const double r0 = -shf(ia[6], 0), r1 = -shf(ia[7], 0), r2 = -shf(ia[8], 0);
 #endif
+        const double i0 = 1.0 / a, l10 = bx * i0, l20 = by * i0;
+        const double d1 = cxx - l10 * bx, i1 = 1.0 / d1, t21 = cxy - l20 * bx, l21 = t21 * i1;
+        const double d2 = cyy - l20 * by - l21 * t21, i2 = 1.0 / d2;
+        const double y0 = r0, y1 = r1 - l10 * y0, y2 = r2 - l20 * y0 - l21 * y1;
+        a2 = y2 * i2; a1 = y1 * i1 - l21 * a2; a0 = y0 * i0 - l10 * a1 - l20 * a2;
+    }
+    chain_outward(xs, ch, a0, a1, a2);
+    TRL_CLK_END(ph_out, clk);
+}
 
 // ================================================================================================ controller half
 // Returns the clamped joint torque of link `lane` (0 for the root and idle lanes).
@@ -631,8 +787,10 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
                                     double h, int contact) {
     const double lk_mass = lc.mass;      // read once (shared-memory table; a read cannot move across the shuffles below)
     const ModelConst& m = c_model;
-    const int nj = m.nj, nd = m.ndof, md = m.max_depth;
-    double* M = xs + X_M;
+    const int md = m.max_depth;
+    const ChainC ch = chain_of(lc);
+    double* slot = xs + X_LNK + lane * kLinkStride;     // this link's slot of the link block (written by active link lanes only)
+    TRL_CLK_BEGIN(clk);
 
     // ---- body inertia about O in world axes, RNEA accelerations with qdd = 0 and the reference's Cj
     const double hx = lk_mass * k.cx, hy = lk_mass * k.cy, Io = lc.izz_c + lk_mass * (k.cx * k.cx + k.cy * k.cy);
@@ -664,43 +822,17 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
         if (!lc.act) { vals[4] = vals[5] = vals[6] = 0.0; }
     }
     {
-        const unsigned long long acc_src_v = lc.acc_src;       // one read of the schedule word, not one per round
-        for (int r = 0; r < m.acc_rounds; ++r) TRL_ACCUM_ROUND(r, 7, vals);
+        if (lc.act) store_vals(slot, vals);
+        __syncwarp();
+        double sum[7];
+        chain_inward<7, false>(xs, ch, lane, 0.0, sum);
+        if (lc.act) load_vals(slot, vals);
     }
+    TRL_CLK_END(PH_RNEA, clk);
     const double s1 = k.ry, s2 = -k.rx;                       // S_j = (1, s1, s2)
     // bias force C (per link lane; the root's three entries live in lane 0)
     const double Cj = vals[4] + s1 * vals[5] + s2 * vals[6];
     const double C0 = shf(vals[5], 0), C1 = shf(vals[6], 0), C2 = shf(vals[4], 0);
-
-    // ---- CRBA: M[i][a] = S_a . (Ic_i S_i) for every ancestor a of i; lower triangle in shared memory
-    for (int t = lane; t < kTri; t += kWarp) M[t] = 0.0;
-    __syncwarp();
-    {
-        const double Fn = vals[0] - vals[2] * s1 + vals[1] * s2;      // Ic = [[I, -hy, hx], [-hy, m, 0], [hx, 0, m]]
-        const double Fx = -vals[2] + vals[3] * s1, Fy = vals[1] + vals[3] * s2;
-        const int dj = lane + 2;
-        bool walking = lc.act && lane > 0;
-        if (walking) M[tri(dj, dj)] = Fn + s1 * Fx + s2 * Fy;
-        int cur = lc.parent;
-        for (int it = 0; it < md; ++it) {
-            double cry = shf(k.ry, cur), crx = shf(k.rx, cur);
-            int cpar = shfi(lc.parent, cur);
-            if (walking) {
-                if (cur > 0) {
-                    M[tri(dj, cur + 2)] = Fn + cry * Fx - crx * Fy;
-                    cur = cpar;
-                } else {
-                    M[tri(dj, 0)] = Fx; M[tri(dj, 1)] = Fy; M[tri(dj, 2)] = Fn;
-                    walking = false;
-                }
-            }
-        }
-        if (lane == 0) {
-            M[tri(0, 0)] = vals[3]; M[tri(1, 1)] = vals[3];
-            M[tri(2, 0)] = -vals[2]; M[tri(2, 1)] = vals[1]; M[tri(2, 2)] = vals[0];
-        }
-    }
-    __syncwarp();
 
     // ---- ApplyFeedback (sim/DogController.cpp:903-945) / ApplySwingFeedback (sim/RaptorController.cpp:907-931)
     const int state = L.i(I_STATE);
@@ -750,87 +882,27 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
         tau0 = pd_on ? (LT(kp, lane) * (perr - h * e.qd) + kd_link * verr) : 0.0;
         rhs_link = tau0 - Cj;
     }
-    // dof-lane view: lane d holds row d of (M + h Kd) and rhs_d
-    double rhs = shf(rhs_link, lane >= 2 ? lane - 2 : 0);
-    double kdd = shf(kd_link, lane >= 2 ? lane - 2 : 0);
-    if (lane == 0) { rhs = -C0; kdd = 0.0; }
-    else if (lane == 1) { rhs = -C1; kdd = 0.0; }
-    else if (lane == 2) { rhs = -C2; kdd = 0.0; }
-    else if (lane >= nd) { rhs = 0.0; kdd = 0.0; }
-    double row[kMaxDof];
-#pragma unroll
-    for (int c = 0; c < kMaxDof; ++c) row[c] = (lane < nd && c <= lane) ? M[tri(lane < nd ? lane : 0, c <= lane ? c : 0)] : 0.0;
-    {
-        double dadd = h * kdd;
-#pragma unroll
-        for (int c = 0; c < kMaxDof; ++c) if (c == lane) row[c] += dadd;
+    // (M + h Kd) acc = rhs is the articulated-body problem of the same tree at rest: no velocity products, no gravity, joint
+    // forces rhs_j, the root's generalised force (-C0, -C1, -C2) as the spatial force (n, fx, fy) = (-C2, -C0, -C1) (a bias
+    // force is its negative), and h kd_j as a joint armature added to D_j -- O(n) instead of the dense 23x23 factorisation
+    if (lc.act) {
+        const double own[9] = {Io, -hy, hx, lk_mass, 0.0, lk_mass, lane == 0 ? C2 : 0.0, lane == 0 ? C0 : 0.0, lane == 0 ? C1 : 0.0};
+        store_vals(slot, own);
+        slot[LK_TAU] = rhs_link;
+        *trl_as2<double2>(slot + LK_CV) = make_double2(0.0, 0.0);
+        *trl_as2<double2>(slot + LK_S) = make_double2(s1, s2);
+        *trl_as2<double2>(slot + LK_LIM) = make_double2(0.0, kd_link);
     }
-    // register-resident LDL^T: pivot broadcast by shuffle, trailing update predicated on lane >= column
-    double diag = 1.0;
-#if TRL_LDLT_SMEM
-    // Experiment: the pivot column travels through shared memory -- every lane stores its A_ij once, all lanes read the column
-    // entries as broadcast 128-bit loads -- and the forward substitution rides along (y_j is final at step j).  Same
-    // operations in the same order per lane as the shuffle form below, so the results are bit-identical.
-    double y = rhs;
-#pragma unroll
-    for (int j = 0; j < kMaxDof; ++j) {
-        double* col = xs + X_COL + (j & 1) * kColStride;
-        col[lane] = row[j];
-        if (lane == j) col[kWarp] = y;
-        __syncwarp();
-        double dj = col[j];
-        if (j >= nd) dj = 1.0;
-        const double inv = 1.0 / dj;
-        if (lane == j) diag = dj;
-        const double lij = row[j] * inv;
-#pragma unroll
-        for (int c0 = (j + 1) & ~1; c0 < kMaxDof; c0 += 2) {
-            const double2 t = *trl_as2<const double2>(col + c0);
-            if (c0 > j && lane >= c0) row[c0] -= lij * t.x;
-            if (c0 + 1 < kMaxDof && lane >= c0 + 1) row[c0 + 1] -= lij * t.y;
-        }
-        const double yj = col[kWarp];
-        if (lane > j) { y -= lij * yj; row[j] = lij; }
-    }
-    y /= diag;
-#else
-#pragma unroll
-    for (int j = 0; j < kMaxDof; ++j) {
-        double dj = shf(row[j], j);
-        if (j >= nd) dj = 1.0;            // padding rows of a smaller character (raptor: 21 dof)
-        double inv = 1.0 / dj;
-        if (lane == j) diag = dj;
-        double aij = row[j];              // A_ij before scaling (valid for lanes i > j)
-        double lij = aij * inv;
-#pragma unroll
-        for (int c = j + 1; c < kMaxDof; ++c) {
-            double akj = shf(aij, c);     // A_cj held by lane c
-            if (lane >= c) row[c] -= lij * akj;
-        }
-        if (lane > j) row[j] = lij;
-    }
-    // forward substitution L y = rhs, then D, then L^T x = y (L^T read back from shared memory)
-    double y = rhs;
-#pragma unroll
-    for (int c = 0; c < kMaxDof; ++c) {
-        double yc = shf(y, c);
-        if (lane > c) y -= row[c] * yc;
-    }
-    y /= diag;
-#endif
-#pragma unroll
-    for (int c = 0; c < kMaxDof; ++c) if (lane < nd && c < lane) M[tri(lane, c)] = row[c];
     __syncwarp();
-    double acc = y;
-    for (int c = nd - 1; c >= 1; --c) {
-        double xc = shf(acc, c);
-        if (lane < c) acc -= M[tri(c, lane)] * xc;
-    }
+    TRL_CLK_END(PH_SOLVE, clk);          // feedback laws + the link block; chain_aba counts its own parts, once
     double tau = 0.0;
     {
-        double acc_link = shf(acc, lane + 2 < kWarp ? lane + 2 : 0);
-        if (lc.act && lane > 0) tau = tau0 - kd_eff * h * acc_link;
+        double b0, b1, b2;
+        chain_aba(xs, ch, lane, h, b0, b1, b2 TRL_CLK_ARG(PH_SOLVE, PH_SOLVE));
+        TRL_CLK_RESET(clk);
+        if (lc.act && lane > 0) tau = tau0 - kd_eff * h * slot[LK_QDD];
     }
+    TRL_CLK_END(PH_SOLVE, clk);
 
     // ---- ApplyGravityCompensation (sim/DogController.cpp:947-995, 1120-1175; sim/RaptorController.cpp:983-1026)
     // effector 0 / 1: dog back foot (toe) / front foot (finger); raptor right / left toe.  A dog foot supports when
@@ -950,7 +1022,7 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
         double lim = LT(torque_lim, lane);
         if (fabs(tau) > lim) tau *= lim / fabs(tau);
     } else tau = 0.0;
-    (void)nj;
+    TRL_CLK_END(PH_CTRL_REST, clk);
     return tau;
 }
 
@@ -958,14 +1030,14 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
 // One sub-step of articulated-body forward dynamics with linearly-implicit contact / joint-limit terms.
 // Updates e (q, qd, root translation) in place and returns the contact bitmask (same value in every lane).
 __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g, const double* s_clx, const double* s_cly,
-                               const int* s_cbody, int lane, double dt, double clear_y TRL_PHYS_XS_DECL TRL_REUSE_KIN_DECL) {
+                               const int* s_cbody, int lane, double dt, double clear_y, double* xs TRL_REUSE_KIN_DECL) {
     const double lk_mass = lc.mass;      // read once (shared-memory table; a read cannot move across the shuffles below)
     // per-body box tables (link frame): centre offset, axis rotation, half sizes -- staged by the kernel next to the corner tables
     const double *s_bax = s_clx + 4 * kMaxJoints, *s_bay = s_bax + kMaxJoints, *s_bc = s_bay + kMaxJoints, *s_bs = s_bc + kMaxJoints,
                  *s_hx = s_bs + kMaxJoints, *s_hy = s_hx + kMaxJoints;
     const ModelConst& m = c_model;
     const PhysParams& pp = m.phys;
-    const int md = m.max_depth;
+    TRL_CLK_BEGIN(clk);
 #if TRL_REUSE_KIN
     Kin k;
     if (k0) k = *k0; else k = kinematics(lc, e TRL_KIN_XS_ARG);
@@ -985,6 +1057,7 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
         if (!lc.act) { ia[6] = ia[7] = ia[8] = 0.0; }
     }
     const double cvx = e.qd * (k.w * k.rx + k.vy), cvy = e.qd * (k.w * k.ry - k.vx);   // c_j = v_j x (S_j qd_j)
+    TRL_CLK_END(PH_KIN, clk);
 
     // ---- contacts: one box corner per lane per round against the height field
     int contact = 0;
@@ -1149,105 +1222,30 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
         if (mine && ((tmask >> (cb - base)) & 0xfu)) contact |= 1 << lane;
     }
     contact = (int)__ballot_sync(kFull, contact != 0);   // lane index == link index
+    TRL_CLK_END(PH_CONTACT, clk);
 
-    // ---- pass 2: articulated inertias / bias forces inward (level-synchronous)
-    const double s1 = k.ry, s2 = -k.rx;
-    double U0 = 0.0, U1 = 0.0, U2 = 0.0, dinv = 0.0, uu = 0.0;
-    // one-sided implicit spring-damper at the joint limits (branch-free: the range of a free joint is infinite).  It depends on
-    // the joint's own state only, so it is evaluated once per sub-step, not once per elimination round
-#ifndef TRL_HOIST_LIMITS
-#define TRL_HOIST_LIMITS 1
-#endif
-    const unsigned long long acc_src_v = lc.acc_src;
-#if TRL_HOIST_LIMITS
+    // ---- articulated-body forward dynamics over the chain schedule
+    // one-sided implicit spring-damper at the joint limits (branch-free: the range of a free joint is infinite)
     const double viol = fmax(e.q - lc.lim_hi, 0.0) + fmin(e.q - lc.lim_lo, 0.0);
     const double cl = (viol != 0.0) ? pp.d_lim + dt * pp.k_lim : 0.0;
     const double lim_f = pp.k_lim * viol + cl * e.qd;
-    const int my_round = lc.acc_round;
-#else
-#define my_round lc.acc_round
-#endif
-    for (int r = 0; r < m.acc_rounds; ++r) {
-        if (my_round == r) {
-            U0 = ia[0] + ia[1] * s1 + ia[2] * s2;
-            U1 = ia[1] + ia[3] * s1 + ia[4] * s2;
-            U2 = ia[2] + ia[4] * s1 + ia[5] * s2;
-            double Dj = U0 + s1 * U1 + s2 * U2;
-            uu = e.tau - (ia[6] + s1 * ia[7] + s2 * ia[8]);
-#if !TRL_HOIST_LIMITS
-            const double viol = fmax(e.q - lc.lim_hi, 0.0) + fmin(e.q - lc.lim_lo, 0.0);
-            const double cl = (viol != 0.0) ? pp.d_lim + dt * pp.k_lim : 0.0;
-            const double lim_f = pp.k_lim * viol + cl * e.qd;
-#endif
-            uu -= lim_f;
-            Dj += dt * cl;
-            dinv = 1.0 / Dj;
-            // Ia = IA - U U^T / D ;  pa = pA + Ia c + U u / D
-            double n0 = ia[0] - U0 * U0 * dinv, n1 = ia[1] - U0 * U1 * dinv, n2 = ia[2] - U0 * U2 * dinv;
-            double n3 = ia[3] - U1 * U1 * dinv, n4 = ia[4] - U1 * U2 * dinv, n5 = ia[5] - U2 * U2 * dinv;
-            double ud = uu * dinv;
-            ia[6] += n1 * cvx + n2 * cvy + U0 * ud;
-            ia[7] += n3 * cvx + n4 * cvy + U1 * ud;
-            ia[8] += n4 * cvx + n5 * cvy + U2 * ud;
-            ia[0] = n0; ia[1] = n1; ia[2] = n2; ia[3] = n3; ia[4] = n4; ia[5] = n5;
-        }
-        TRL_ACCUM_ROUND(r, 9, ia);
+    double* slot = xs + X_LNK + lane * kLinkStride;
+    if (lc.act) {
+        store_vals(slot, ia);
+        slot[LK_TAU] = e.tau;
+        *trl_as2<double2>(slot + LK_CV) = make_double2(cvx, cvy);
+        *trl_as2<double2>(slot + LK_S) = make_double2(k.ry, -k.rx);
+        *trl_as2<double2>(slot + LK_LIM) = make_double2(lim_f, cl);
     }
-    // floating base: solve IA_0 a_0 = -pA_0 (symmetric 3x3 LDL^T); every lane computes it from lane 0's values
-    double a0, a1, a2;
-    {
-#if TRL_OUTWARD_SMEM
-        double* bs = xs + X_BASE;
-        if (lane == 0) {
-            double2* b2 = trl_as2<double2>(bs);
-            b2[0] = make_double2(ia[0], ia[1]); b2[1] = make_double2(ia[2], ia[3]); b2[2] = make_double2(ia[4], ia[5]);
-            b2[3] = make_double2(ia[6], ia[7]); bs[8] = ia[8];
-        }
-        __syncwarp();
-        const double2 q0 = trl_as2<const double2>(bs)[0], q1 = trl_as2<const double2>(bs)[1],
-                      q2 = trl_as2<const double2>(bs)[2], q3 = trl_as2<const double2>(bs)[3];
-        double a = q0.x, bx = q0.y, by = q1.x, cxx = q1.y, cxy = q2.x, cyy = q2.y;
-        double r0 = -q3.x, r1 = -q3.y, r2 = -bs[8];
-#else
-        double a = shf(ia[0], 0), bx = shf(ia[1], 0), by = shf(ia[2], 0), cxx = shf(ia[3], 0), cxy = shf(ia[4], 0), cyy = shf(ia[5], 0);
-        double r0 = -shf(ia[6], 0), r1 = -shf(ia[7], 0), r2 = -shf(ia[8], 0);
-#endif
-        const double i0 = 1.0 / a, l10 = bx * i0, l20 = by * i0;
-        const double d1 = cxx - l10 * bx, i1 = 1.0 / d1, t21 = cxy - l20 * bx, l21 = t21 * i1;
-        const double d2 = cyy - l20 * by - l21 * t21, i2 = 1.0 / d2;
-        const double y0 = r0, y1 = r1 - l10 * y0, y2 = r2 - l20 * y0 - l21 * y1;
-        a2 = y2 * i2; a1 = y1 * i1 - l21 * a2; a0 = y0 * i0 - l10 * a1 - l20 * a2;
-    }
-    // pass 3: accelerations outward; each link lane integrates its own joint (semi-implicit Euler)
-    double aw = a0, alx = a1, aly = a2;
     const double thd0 = shf(e.qd, 0);
-#if TRL_HOIST_LIMITS
-    const int my_depth = lc.depth, my_parent = lc.parent;
-#else
-#undef my_round
-#define my_depth lc.depth
-#define my_parent lc.parent
-#endif
-    for (int l = 1; l <= md; ++l) {
-#if TRL_OUTWARD_SMEM
-        // every lane publishes its current (aw, ax, ay); a link of depth l reads its parent's, which is final since level l-1.
-        // Levels alternate between two buffers: one barrier per level (see TRL_TREE_PREFIX2)
-        double2* o2 = trl_as2<double2>(xs + X_OUT + (l & 1) * kOutBuf);
-        double* o1 = xs + X_OUT + (l & 1) * kOutBuf + 2 * kWarp;
-        o2[lane] = make_double2(aw, alx); o1[lane] = aly;
-        __syncwarp();
-        const double2 pp_ = o2[my_parent];
-        const double paw = pp_.x, pax = pp_.y, pay = o1[my_parent];
-#else
-        double paw = shf(aw, my_parent), pax = shf(alx, my_parent), pay = shf(aly, my_parent);
-#endif
-        if (my_depth == l) {
-            double bx = pax + cvx, by = pay + cvy;
-            double qdd = (uu - (U0 * paw + U1 * bx + U2 * by)) * dinv;
-            aw = paw + qdd; alx = bx + s1 * qdd; aly = by + s2 * qdd;
-            e.qd += dt * qdd;
-            e.q += dt * e.qd;
-        }
+    __syncwarp();
+    TRL_CLK_END(PH_INWARD, clk);
+    double a0, a1, a2;
+    chain_aba(xs, chain_of(lc), lane, dt, a0, a1, a2 TRL_CLK_ARG(PH_INWARD, PH_OUTWARD));
+    // each link lane integrates its own joint (semi-implicit Euler)
+    if (lc.act && lane > 0) {
+        e.qd += dt * slot[LK_QDD];
+        e.q += dt * e.qd;
     }
     {
         // root: classical acceleration of the origin = spatial acceleration + w x v
@@ -1256,10 +1254,7 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
         e.ox += dt * e.oxd; e.oy += dt * e.oyd;
         if (lane == 0) { e.qd += dt * a0; e.q += dt * e.qd; }
     }
-#if !TRL_HOIST_LIMITS
-#undef my_depth
-#undef my_parent
-#endif
+    TRL_CLK_RESET(clk);
     return contact;
 }
 
@@ -1372,11 +1367,8 @@ __global__ void __launch_bounds__(kBlockThreads, TRL_STEP_MIN_BLOCKS)
 trl_step_kernel(Buffers B, double h, int flags, int lists) {
     __shared__ double s_clx[4 * kMaxJoints + 6 * kMaxJoints], s_cly[4 * kMaxJoints];     // s_clx also carries the six per-body box tables
     __shared__ int s_cbody[4 * kMaxJoints];
-#if TRL_SMEM_ALIGNED
     __shared__ __align__(16) double s_x[kWarpsPerBlock * X_END];
-#else
-    __shared__ double s_x[kWarpsPerBlock * X_END];
-#endif
+    TRL_CLK_BEGIN(clk);
     const ModelConst& m = c_model;
     for (int t = threadIdx.x; t < m.n_corners; t += kBlockThreads) {
         s_clx[t] = LT(corner_lx, t); s_cly[t] = LT(corner_ly, t); s_cbody[t] = LT(corner_body, t);
@@ -1451,6 +1443,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
     EnvRegs e;
     load_env(L, lc, e, lane);
     int contact = L.i(I_CONTACT);
+    TRL_CLK_END(PH_LOAD, clk);
 
 #if TRL_REUSE_KIN
     Kin k_ctrl;
@@ -1468,7 +1461,9 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
 #if TRL_REUSE_KIN
         k_ctrl = k; have_k = true;
 #endif
+        TRL_CLK_END(PH_KIN, clk);
         e.tau = controller_torque(L, lc, e, k, xs, lane, h, contact);
+        TRL_CLK_RESET(clk);
         if (lane == 0) {
             // fall checks (sim/SimCharSoftFall.cpp:74-125)
             double cnt = L.d(D_FALL_DIST_CNT) - h;
@@ -1500,6 +1495,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
             if (m.exp_mode) exp_new_cycle_update(L, B, fl != 0, lane);
             else if (lane == 0) L.i(I_CYCLE_COUNT) += 1;
         }
+        TRL_CLK_END(PH_CTRL_REST, clk);
     }
 
     if (flags & 4) {
@@ -1531,6 +1527,10 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
 
     if (flags & 2) {
         // ---------------- physics half of env-step k+1
+#if TRL_PHASE_CLOCKS
+        if (lane == 0) atomicAdd(&g_phase_clocks[kNumPhases], 1ull);
+#endif
+        TRL_CLK_END(PH_TAIL, clk);
         GroundView g = load_ground(L, B);
         const int ns = m.num_sim_substeps;
         const double dt = h / ns;
@@ -1539,10 +1539,11 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         const double clear_y = g.window_max(e.ox - m.reach - 0.25, e.ox + m.reach + 0.25, lane) + kClearMargin;
 #if TRL_REUSE_KIN
         for (int s = 0; s < ns; ++s)
-            contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y TRL_PHYS_XS_ARG, (s == 0 && have_k) ? &k_ctrl : nullptr);
+            contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y, xs, (s == 0 && have_k) ? &k_ctrl : nullptr);
 #else
-        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y TRL_PHYS_XS_ARG);
+        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y, xs);
 #endif
+        TRL_CLK_RESET(clk);
         // UpdateGround (scenarios/ScenarioSimChar.cpp:564-572): regenerate a segment when the view window crosses it
         {
             int smin = g.seg_id(0), smax = g.seg_id(1);
@@ -1607,6 +1608,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
                 B.pending_list[app * B.n + slot] = env;
             }
         }
+        TRL_CLK_END(PH_TAIL, clk);
     }
     }   // rep
     store_env(L, lc, e, lane);
@@ -1615,6 +1617,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
     for (int f = lane; f < D_NUM_FIELDS; f += kWarp) L.D[(size_t)f * L.n + env] = L.sd[f];
     if (lane < I_NUM_FIELDS) L.I[(size_t)lane * L.n + env] = L.si[lane];
 #endif
+    TRL_CLK_END(PH_LOAD, clk);
     if (flags & kStepCatchUp) catchup_leave(B, prev);
 }
 
@@ -1713,11 +1716,30 @@ cudaError_t upload_model(const ModelConst& mc) {
     return e;
 }
 size_t step_smem_bytes() { return 0; }
+// TRL_PHASE_CLOCKS builds: copy the accumulated phase clocks (kNumPhases + the env-step count) into out[], optionally zero them
+cudaError_t step_phase_clocks(unsigned long long* out, int reset) {
+#if TRL_PHASE_CLOCKS
+    cudaError_t e = cudaMemcpyFromSymbol(out, g_phase_clocks, sizeof(g_phase_clocks));
+    if (e == cudaSuccess && reset) {
+        const unsigned long long zero[kNumPhases + 1] = {};
+        e = cudaMemcpyToSymbol(g_phase_clocks, zero, sizeof(zero));
+    }
+    return e;
+#else
+    (void)out; (void)reset;
+    return static_cast<cudaError_t>(1);   // not a measurement build
+#endif
+}
 cudaError_t configure_step_kernels() {
-#if TRL_SMEM_ALIGNED && !defined(TRL_SIMT_EMU)
-    // experiment builds stage lane-to-lane exchanges in shared memory (up to 42 KB per CTA): ask for the largest carve-out so
-    // that the register-limited 4 CTAs per SM still fit
-    return cudaFuncSetAttribute(trl_step_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+#if !defined(TRL_SIMT_EMU)
+    // the per-warp link blocks take the CTA's static shared memory to ~25 KB: ask for a carve-out that holds the
+    // TRL_STEP_MIN_BLOCKS CTAs per SM the register budget is sized for (+1 KB the system reserves per CTA), and no more (L1)
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, trl_step_kernel);
+    if (e != cudaSuccess) return e;
+    const double need = (double)TRL_STEP_MIN_BLOCKS * (double)(fa.sharedSizeBytes + 1024);
+    const int pct = std::min(100, (int)std::ceil(100.0 * need / (228.0 * 1024.0)));
+    return cudaFuncSetAttribute(trl_step_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
 #else
     return cudaSuccess;
 #endif

@@ -96,11 +96,16 @@ struct ModelConst {
     int depth[kMaxJoints], max_depth;
     int child[kMaxJoints][4];              // up to 4 children per link (-1 = none)
     int anc_pow[kMaxJoints][4];            // 2^k-th ancestor of each link (k = 0..3), -1 if it does not exist
-    // inward (leaf -> root) pass schedule: link j is eliminated in round acc_round[j] and handed to its parent at the end
-    // of that round; siblings get distinct rounds so that every lane receives from at most ONE lane per round.
-    // acc_src[j] packs, 5 bits per round, the lane that lane j receives from (31 = none: lane 31 is idle and holds zeros)
-    int acc_round[kMaxJoints], acc_rounds;
-    unsigned long long acc_src[kMaxJoints];
+    // chain schedule of the tree recursions (inward sums / eliminations, outward accelerations): the tree is split into chains,
+    // maximal runs of single-child links from a leaf or a branch point up to the child of the next branch point.  Lane c walks
+    // chain c (chain 0 holds the root); chains of level l only merge chains of lower levels into their bottom link, so a pass is
+    // chain_levels steps of at most chain_level_len[l] links each, with one warp barrier per level.
+    int n_chains, chain_levels;
+    int chain_level_len[kMaxJoints];
+    unsigned long long chain_links[kMaxJoints];   // 5 bits per link, bottom link first
+    int chain_len[kMaxJoints], chain_level[kMaxJoints];
+    int chain_merge[kMaxJoints];           // 5 bits per child chain summed into the bottom link, in summation order (31 = none)
+    int chain_up[kMaxJoints];              // parent link of the chain's top link (-1 for the root's chain)
     int n_corners;                         // 4 * number of collidable bodies
     int corner_body[4 * kMaxJoints];
     double corner_lx[4 * kMaxJoints], corner_ly[4 * kMaxJoints];   // corner position in the link (joint) frame

@@ -23,25 +23,22 @@ NVCC_FLAGS = ARCH_FLAGS + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPI
 # the environment of a measurement run; every variant is the same CUDA path compiled with one more -D flag and lives beside
 # the product library (lib/variants/<name>/).  Unset = the product build.  There is still no CPU path behind any of them.
 VARIANTS = {
-    "accum_smem": ["-DTRL_ACCUM_SMEM=1"],
-    "ldlt_regs": ["-DTRL_LDLT_SMEM=0"],          # the round-1 default: pivot column exchanged by shuffles
     "kin_smem": ["-DTRL_KIN_SMEM=1"],
-    "outward_smem": ["-DTRL_OUTWARD_SMEM=1"],
+    "outward_smem": ["-DTRL_OUTWARD_SMEM=1"],    # since the chain passes: only the floating-base broadcast (parent -> child accelerations always use the link block)
     "contact_smem": ["-DTRL_CONTACT_SMEM=1"],
-    "accum_ldlt": ["-DTRL_ACCUM_SMEM=1"],                                  # the two largest families, 23 KB smem / CTA
-    "xchg_no_contact": ["-DTRL_ACCUM_SMEM=1", "-DTRL_LDLT_SMEM=1", "-DTRL_KIN_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],   # 36 KB
+    "xchg_no_contact": ["-DTRL_KIN_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],
     "smem_xchg": ["-DTRL_SMEM_XCHG=1"],
     "smem_xchg_3cta": ["-DTRL_SMEM_XCHG=1", "-DTRL_STEP_MIN_BLOCKS=3"],
     "noinline_cold": ["-DTRL_NOINLINE_COLD=1"],
     "regs96": ["-DTRL_STEP_MIN_BLOCKS=5"],       # 5 CTAs (20 warps) per SM at 96 registers, more spills; only makes sense with env groups
     "regs80": ["-DTRL_STEP_MIN_BLOCKS=6"],
+    "phase_clocks": ["-DTRL_PHASE_CLOCKS=1"],    # per-phase clock64() sums of the step kernel (tools/step_phase_probe.py)
     "field_smem": ["-DTRL_FIELD_SMEM=1"],        # every per-env field staged in shared memory for the launch (one load batch, one store batch): not adopted
     "cta1": ["-DTRL_WARPS_PER_BLOCK=1", "-DTRL_STEP_MIN_BLOCKS=16"],     # CTA size of the step kernel: 1 / 2 / 8 warps (default 4), 16 warps per SM in all
     "cta2": ["-DTRL_WARPS_PER_BLOCK=2", "-DTRL_STEP_MIN_BLOCKS=8"],
     "cta8": ["-DTRL_WARPS_PER_BLOCK=8", "-DTRL_STEP_MIN_BLOCKS=2"],
     "table_const": ["-DTRL_TABLE_MIRROR=0"],     # lane-indexed model tables from constant memory (divergent LDC, the round-1 reads); the default reads a global-memory mirror
-    "no_hoist": ["-DTRL_HOIST_LIMITS=0"],        # joint-limit terms and link indices re-evaluated in every ABA round (the code before the hoist)
-    "contact_outward_smem": ["-DTRL_CONTACT_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],
+    "contact_outward_smem": ["-DTRL_CONTACT_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],   # outward part: the floating-base broadcast only (see outward_smem)
     "link_regs": ["-DTRL_LINK_SMEM=0"],          # the round-1 layout: per-lane link constants in registers (the default keeps them in shared memory)          # per-lane link constants in shared memory instead of ~28 registers (180 B instead of 216 B spilled)
     "reuse_kin": ["-DTRL_REUSE_KIN=1"],
     "smem_xchg_reuse_kin": ["-DTRL_SMEM_XCHG=1", "-DTRL_REUSE_KIN=1"],
@@ -125,7 +122,7 @@ EXPORTS = [
     "trl_set_explore", "trl_set_phys_params", "trl_set_weights", "trl_sizes", "trl_num_tuples", "trl_get_tuples",
     "trl_get_tuples_f64", "trl_reset_tuples", "trl_eval_stats", "trl_dist_log", "trl_reset_avg_dist", "trl_get_state", "trl_set_state",
     "trl_get_state_all", "trl_get_ctrl", "trl_get_poli_state", "trl_get_net_out", "trl_get_layer_state", "trl_get_terrain",
-    "trl_kernel_launches", "trl_last_error", "trl_bench_updates", "trl_update_timed", "trl_device_tuple_block", "trl_snapshot", "trl_snapshot_wait", "trl_update_timed_detail", "trl_update_timeline", "trl_debug_time_decide", "trl_debug_fc_phases",
+    "trl_kernel_launches", "trl_last_error", "trl_bench_updates", "trl_update_timed", "trl_device_tuple_block", "trl_snapshot", "trl_snapshot_wait", "trl_update_timed_detail", "trl_update_timeline", "trl_debug_time_decide", "trl_debug_fc_phases", "trl_debug_step_phases",
     "trl_load_model", "trl_output_model", "trl_write_model", "trl_get_output_offset_scale", "trl_pack_output_offset_scale",
     "trl_set_terrain_lerp", "trl_train_schedule", "trl_trainer_create", "trl_trainer_destroy", "trl_trainer_init_fresh", "trl_trainer_add_from_scene", "trl_trainer_add_tuples", "trl_trainer_add_device", "trl_trainer_train", "trl_train_run", "trl_train_run_timed",
     "trl_trainer_counters", "trl_trainer_num_params", "trl_trainer_launches", "trl_trainer_get", "trl_trainer_set_theta", "trl_trainer_list", "trl_trainer_rows",

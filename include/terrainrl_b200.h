@@ -128,6 +128,10 @@ int trl_update_timeline(trl_handle* h, double dt, double* out4, int cap, int* n)
 int trl_debug_time_decide(trl_handle* h, int n_pending, int iters, double* ms_avg);
 /* measurement only: in-kernel phase stamps (ns from entry, 16 slots) of the batched decision path's FC kernel + event-timed conv / FC launches */
 int trl_debug_fc_phases(trl_handle* h, int n_pending, double* out_ns16, double* conv_us, double* fc_us);
+/* measurement only, TRL_PHASE_CLOCKS=1 builds: clock64() cycles of the env-step kernel summed over warps per phase (9 slots: state
+ * load/store, controller RNEA, mass-matrix solve, rest of the controller, kinematics, contacts, inward pass, base + outward pass,
+ * terrain / FSM / policy state) + out[9] = env-steps counted; n must be 10 */
+int trl_debug_step_phases(trl_handle* h, unsigned long long* out, int n, int reset);
 
 /* ---------------------------------------------------------------------------------------------------------------------
  * MACE trainer on the GPU (SURVEY.md §8 f1) -- replaces cMACETrainer / cNeuralNetLearner behind cScenarioTrainMACE:
