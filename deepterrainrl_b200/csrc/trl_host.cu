@@ -365,12 +365,8 @@ static int upload_net(trl_handle* h, const double* const* blobs, const int64_t* 
         CK(cudaMemcpyAsync(h->net_blobs[i], src, (size_t)c * 8, cudaMemcpyHostToDevice, h->stream));
     }
     CK(cudaStreamSynchronize(h->stream));
-    NetWeights& W = h->W;
     double** b = h->net_blobs.data();
-    W.conv0_w = b[0]; W.conv0_b = b[1]; W.conv1_w = b[2]; W.conv1_b = b[3]; W.conv2_w = b[4]; W.conv2_b = b[5];
-    W.tip0_w = b[6]; W.tip0_b = b[7]; W.ip0_w = b[8]; W.ip0_b = b[9];
-    for (int k = 0; k < 4; ++k) { W.h0_w[k] = b[10 + 4 * k]; W.h0_b[k] = b[11 + 4 * k]; W.h1_w[k] = b[12 + 4 * k]; W.h1_b[k] = b[13 + 4 * k]; }
-    W.in_off = b[26]; W.in_scale = b[27]; W.out_off = b[28]; W.out_scale = b[29];
+    h->W = net_weights(b, b[26], b[27], b[28], b[29]);
     return 0;
 }
 

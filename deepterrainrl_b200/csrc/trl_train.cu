@@ -36,7 +36,6 @@ using namespace trl;
 
 constexpr int kB = 32;                               // MemoryData batch_size
 constexpr int C0 = 16, K0 = 8, W0 = 193, C1 = 32, K1 = 4, W1 = 190, C2 = 32, K2 = 4, W2 = 187, T = 64, H = 256, HH = 128;
-constexpr int kSplit = 8;                            // K slices of the wide terr_ip0 forward
 constexpr int kTerr = 200;                           // terrain samples at the head of the policy state
 
 enum Pred { P_ALWAYS = 0, P_CRITIC, P_CAND, P_ACTOR, P_INIT };
@@ -62,7 +61,7 @@ struct Dev {
     double *xn, *a0, *a1, *a2, *t, *catb, *h, *hh, *y;           // activations of the most recent forward pass (kB rows)
     double *v0, *v1;
     double *dy, *dhh, *dh, *dt, *da2, *da1, *da0;
-    double *mean, *part;
+    double* mean;
     double discount, base_lr, momentum, weight_decay;
     int freeze, nis, init_offset_scale, steps_per_iter;
     unsigned long long rng_key;
@@ -71,7 +70,7 @@ struct Dev {
 // Programmatic dependent launch: every trainer kernel is launched with programmatic stream serialization and starts with
 // pdl_sync(): wait until the preceding kernel has completed (and its writes are visible), then let the next kernel of the
 // stream be scheduled right away -- it parks at its own wait.  The dependency chain stays strictly serial; what disappears is
-// the launch latency between ~140 small dependent kernels per training iteration.
+// the launch latency between the small dependent kernels of a training iteration (40 at one step per iteration).
 __device__ __forceinline__ void pdl_sync() {
 #ifndef TRL_SIMT_EMU   // the test-only emulator runs launches strictly in order
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -547,111 +546,6 @@ __global__ void k_gather_norm(Dev d, int pred, int col0, int col1, int col2, int
     const float* r = d.mem + (size_t)ids[n % kB] * d.Wd + (b == 0 ? col0 : (b == 1 ? col1 : col2));
     for (int i = threadIdx.x; i < d.S; i += blockDim.x) d.xn[(size_t)n * d.S + i] = ((double)r[i] + in_off[i]) * in_scale[i];
 }
-// Convolution (cross-correlation, stride 1) + ReLU.  grid (cout / kConvOut, kB): the block stages all input channels of its
-// sample in (dynamic) shared memory once and produces kConvOut output channels from it, one thread per output position.
-constexpr int kConvOut = 8;
-__global__ void k_conv_fwd(Dev d, int pred, const double* x, int ldn, int cin, int win, const double* w, const double* b, int cout, int k,
-                           double* y) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    TRL_DYN_SHARED(double, xs);                            // [cin][win]
-    __shared__ double ws[kConvOut][C1 * K2];              // cin * k <= 128 per output channel
-    const int o0 = blockIdx.x * kConvOut, n = blockIdx.y, wout = win - k + 1, ck = cin * k;
-    const double* xr = x + (size_t)n * ldn;
-    for (int i = threadIdx.x; i < cin * win; i += blockDim.x) xs[i] = xr[i];
-    for (int i = threadIdx.x; i < kConvOut * ck; i += blockDim.x) { const int j = i / ck, r = i - j * ck; ws[j][r] = w[(size_t)(o0 + j) * ck + r]; }
-    __syncthreads();
-    const int t = threadIdx.x;
-    if (t >= wout) return;
-    double acc[kConvOut];
-#pragma unroll
-    for (int j = 0; j < kConvOut; ++j) acc[j] = b[o0 + j];
-    for (int c = 0; c < cin; ++c)
-        for (int kk = 0; kk < k; ++kk) {
-            const double xv = xs[c * win + t + kk];
-#pragma unroll
-            for (int j = 0; j < kConvOut; ++j) acc[j] += ws[j][c * k + kk] * xv;
-        }
-#pragma unroll
-    for (int j = 0; j < kConvOut; ++j) y[((size_t)n * cout + o0 + j) * wout + t] = acc[j] > 0 ? acc[j] : 0;
-}
-// Narrow InnerProduct layers (nin <= 256): one warp per output neuron, lane = batch row, no reduction.  The block stages
-// 64-column tiles of the kB x nin input (transposed) and of its 8 weight rows in shared memory with coalesced loads; the inner
-// loop runs out of shared memory only (weight = broadcast read, input = conflict-free read).
-__global__ void k_fc_fwd_rows(Dev d, int pred, const double* x, int ldx, int nin, const double* w, const double* b, int nout, int relu,
-                              double* y, int ldy) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    __shared__ double xs[64][kB + 1];
-    __shared__ double ws[8][64 + 1];
-    const int wq = threadIdx.x >> 5, o = blockIdx.x * 8 + wq, n = threadIdx.x & 31;
-    double a0 = 0, a1 = 0;
-    for (int k0 = 0; k0 < nin; k0 += 64) {
-        const int kt = min(64, nin - k0);
-        for (int idx = threadIdx.x; idx < kB * 64; idx += blockDim.x) {
-            const int r = idx >> 6, kk = idx & 63;
-            if (kk < kt) xs[kk][r] = x[(size_t)r * ldx + k0 + kk];
-        }
-        for (int idx = threadIdx.x; idx < 8 * 64; idx += blockDim.x) {
-            const int r = idx >> 6, kk = idx & 63, oo = blockIdx.x * 8 + r;
-            ws[r][kk] = (oo < nout && kk < kt) ? w[(size_t)oo * nin + k0 + kk] : 0.0;
-        }
-        __syncthreads();
-        int kk = 0;
-        for (; kk + 1 < kt; kk += 2) { a0 += ws[wq][kk] * xs[kk][n]; a1 += ws[wq][kk + 1] * xs[kk + 1][n]; }
-        if (kk < kt) a0 += ws[wq][kk] * xs[kk][n];
-        __syncthreads();
-    }
-    if (o >= nout) return;
-    const double s = b[o] + (a0 + a1);
-    y[(size_t)n * ldy + o] = (relu && s < 0) ? 0 : s;
-}
-// Wide InnerProduct (terr_ip0, nin = 5984): K split over blockIdx.y, partial sums [ks][kB][nout] reduced (with bias + ReLU) by
-// k_fc_split_finish in a fixed order.
-__global__ void k_fc_fwd_split(Dev d, int pred, const double* x, int ldx, int nin, const double* w, int nout, double* part) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    const int o = blockIdx.x, ks = blockIdx.y, nks = gridDim.y, tid = threadIdx.x;
-    const int chunk = (nin + nks - 1) / nks, k0 = ks * chunk, k1 = min(nin, k0 + chunk);
-    double acc[kB];
-#pragma unroll
-    for (int n = 0; n < kB; ++n) acc[n] = 0.0;
-    const double* wr = w + (size_t)o * nin;
-    for (int i = k0 + tid; i < k1; i += blockDim.x) {
-        const double wv = wr[i];
-#pragma unroll
-        for (int n = 0; n < kB; ++n) acc[n] += wv * x[(size_t)n * ldx + i];
-    }
-    __shared__ double red[8][kB];
-#pragma unroll
-    for (int n = 0; n < kB; ++n) {
-        double v = warp_sum(acc[n]);
-        if ((tid & 31) == 0) red[tid >> 5][n] = v;
-    }
-    __syncthreads();
-    if (tid < kB) {
-        double s = 0;
-        for (int wq = 0; wq < (int)(blockDim.x >> 5); ++wq) s += red[wq][tid];
-        part[((size_t)ks * kB + tid) * nout + o] = s;
-    }
-}
-__global__ void k_fc_split_finish(Dev d, int pred, const double* part, int nks, const double* b, int nout, int relu, double* y, int ldy) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    const int n = blockIdx.x;
-    for (int o = threadIdx.x; o < nout; o += blockDim.x) {
-        double s = b[o];
-        for (int ks = 0; ks < nks; ++ks) s += part[((size_t)ks * kB + n) * nout + o];
-        y[(size_t)n * ldy + o] = (relu && s < 0) ? 0 : s;
-    }
-}
-__global__ void k_concat(Dev d, int pred) {
-    pdl_sync();        // concat0: [terr_relu3 | char features]
-    if (!pred_on(d, pred)) return;
-    const int n = blockIdx.x;
-    for (int i = threadIdx.x; i < d.cat; i += blockDim.x)
-        d.catb[(size_t)n * d.cat + i] = i < T ? d.t[(size_t)n * T + i] : d.xn[(size_t)n * d.S + kTerr + (i - T)];
-}
 
 // ================================================================================================ labels + loss
 // max over the critic outputs of the un-normalised target-net output (GetMaxFragValAux) -> v0 (state begin) or the Bellman
@@ -702,8 +596,8 @@ __global__ void k_labels(Dev d, int pred, int mode) {
 }
 
 // ================================================================================================ backward
-// The four backward kernels are written as bodies over explicit block / thread coordinates: the per-layer kernels below call one
-// body each, k_bwd_multi (further down) runs several independent bodies in ONE launch (blocks of 256 threads).
+// The four backward operations are written as bodies over explicit block / thread coordinates, so that k_bwd_multi (further down)
+// can run several independent bodies in ONE launch (blocks of 256 threads).
 // dw[o][i] = sum_n dy[n][o] x[n][i], db[o] = sum_n dy[n][o].  grid (nout, ceil(nin / nthreads))
 __device__ __forceinline__ void fc_bwd_w_body(int bx, int by, int tid, int nthreads, const double* dy, int ldy, const double* x, int ldx, int nin,
                                               double* dw, double* db) {
@@ -724,14 +618,9 @@ __device__ __forceinline__ void fc_bwd_w_body(int bx, int by, int tid, int nthre
         db[o] = s;
     }
 }
-__global__ void k_fc_bwd_w(Dev d, int pred, const double* dy, int ldy, const double* x, int ldx, int nin, double* dw, double* db) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    fc_bwd_w_body(blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, dy, ldy, x, ldx, nin, dw, db);
-}
 // dx[n][i] (=|+=) mask(act[n][i]) * sum_o dy[n][o] w[o][i] for i < ncols.  grid (ceil(ncols / 32), kB), block (32, 8): the
 // output neurons are split over ty and reduced through shared memory in a fixed order.  `heads` > 1: the sum over several
-// (dy, w) pairs with strides dy_stride / w_stride, accumulated head after head exactly like `heads` launches with accumulate = 1.
+// (dy, w) pairs (dy at stride dy_stride, w from w_heads), accumulated head after head in head order.
 __device__ __forceinline__ void fc_bwd_x_body(int bx, int by, int tx, int ty, const double* dy, int ldy, int nout, const double* w, int nin, int ncols,
                                               const double* act, int lda, double* dx, int ldx, int accumulate, int heads, size_t dy_stride,
                                               const double* const* w_heads) {
@@ -763,12 +652,6 @@ __device__ __forceinline__ void fc_bwd_x_body(int bx, int by, int tx, int ty, co
         if (accumulate) dx[(size_t)n * ldx + i] += acc; else dx[(size_t)n * ldx + i] = acc;
     }
 }
-__global__ void k_fc_bwd_x(Dev d, int pred, const double* dy, int ldy, int nout, const double* w, int nin, int ncols, const double* act,
-                           int lda, double* dx, int ldx, int accumulate) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    fc_bwd_x_body(blockIdx.x, blockIdx.y, threadIdx.x, threadIdx.y, dy, ldy, nout, w, nin, ncols, act, lda, dx, ldx, accumulate, 1, 0, nullptr);
-}
 // dw[o][c][kk] = sum_{n,t} dy[n][o][t] x[n][c][t + kk]; db[o] = sum dy[n][o][t].  grid (cin, cout)
 __device__ __forceinline__ void conv_bwd_w_body(int bx, int by, int tid, int nthreads, const double* dy, int cout, int k, const double* x, int ldn,
                                                 int cin, int win, double* dw, double* db) {
@@ -799,12 +682,6 @@ __device__ __forceinline__ void conv_bwd_w_body(int bx, int by, int tid, int nth
         else if (tid == K0 && c == 0) db[o] = s;
     }
 }
-__global__ void k_conv_bwd_w(Dev d, int pred, const double* dy, int cout, int k, const double* x, int ldn, int cin, int win, double* dw,
-                             double* db) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    conv_bwd_w_body(blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, dy, cout, k, x, ldn, cin, win, dw, db);
-}
 // dx[n][c][s] = mask * sum_{o,kk} dy[n][o][s - kk] w[o][c][kk].  grid (cin, kB), one thread per input position
 __device__ __forceinline__ void conv_bwd_x_body(int bx, int by, int tid, int nthreads, const double* dy, int cout, int k, const double* w, int cin,
                                                 int win, const double* act, double* dx) {
@@ -825,15 +702,9 @@ __device__ __forceinline__ void conv_bwd_x_body(int bx, int by, int tid, int nth
     const size_t idx = ((size_t)n * cin + c) * win + s;
     dx[idx] = (act[idx] > 0) ? acc : 0;
 }
-__global__ void k_conv_bwd_x(Dev d, int pred, const double* dy, int cout, int k, const double* w, int cin, int win, const double* act,
-                             double* dx) {
-    pdl_sync();
-    if (!pred_on(d, pred)) return;
-    conv_bwd_x_body(blockIdx.x, blockIdx.y, threadIdx.x, blockDim.x, dy, cout, k, w, cin, win, act, dx);
-}
-// Several independent backward bodies in one launch (fewer, fatter launches: the per-layer launches of a batch-32 step are bound
-// by launch latency).  Blocks of 256 threads; job q owns `blocks` consecutive blocks,
-// laid out as a gx x gy grid of that body.  Per-element arithmetic and summation order are those of the per-layer kernels.
+// Several independent backward bodies in one launch (fewer, fatter launches: one launch per body and layer of a batch-32 step
+// would be bound by launch latency).  Blocks of 256 threads; job q owns `blocks` consecutive blocks, laid out as a gx x gy grid of
+// that body.  Each body's per-element arithmetic and summation order do not depend on which jobs share its launch.
 enum JobKind { J_FC_BWD_W = 0, J_FC_BWD_X, J_FC_BWD_X_HEADS, J_CONV_BWD_W, J_CONV_BWD_X };
 struct Job {
     int kind, blocks, gx;
@@ -887,11 +758,10 @@ struct trl_trainer {
     Dev d;
     std::vector<void*> allocs;
     cudaGraphExec_t train_graph = nullptr;
+    int64_t graph_launches = 0;        // kernels in train_graph (one training iteration)
     // forward passes run through the batched decision kernels (trl_decide2.cuh): per net the weight views and TMA descriptors
     trl::NetWeights nw[2];             // 0 current net, 1 target net
     trl::FcMaps fmaps[2];
-    bool batched_fwd = true;           // TRL_TRAIN_FWD_V1=1: the per-layer kernels below
-    bool fused_bwd = true;             // TRL_TRAIN_BWD_V1=1: one launch per backward kernel (26 per pass instead of 8)
     double* stage_rows = nullptr;      // device staging for tuples handed in from the host
     uint32_t* stage_flags = nullptr;
     int stage_cap = 0;
@@ -925,45 +795,24 @@ cudaError_t talloc(trl_trainer* t, Tp** p, size_t count) {
 struct NetRef { const double* theta; const double *in_off, *in_scale; };
 
 // forward pass of the kB rows named by d.ids (replay columns starting at col0) through `net`; activations stay in d.*
-// (col1 / col2 >= 0, batched path only: further blocks of kB rows with the columns starting there ride along; bit b of ids2_mask:
-// block b is taken from the candidate ids)
+// (col1 / col2 >= 0: further blocks of kB rows with the columns starting there ride along; bit b of ids2_mask: block b is taken
+// from the candidate ids)
 int enqueue_forward(trl_trainer* t, int pred, int col0, const NetRef& net, cudaStream_t st, bool keep_act = true, int col1 = -1, int col2 = -1,
                     int ids2_mask = 0) {
     const Dev& d = t->d;
-    const double* th = net.theta;
-    auto blob = [&](int b) { return th + d.off[b]; };
     const int rows = kB * (1 + (col1 >= 0 ? 1 : 0) + (col2 >= 0 ? 1 : 0));
     launch_pdl(k_gather_norm, dim3(rows), dim3(128), 0, st, d, pred, col0, col1, col2, ids2_mask, net.in_off, net.in_scale);
-    if (t->batched_fwd) {
-        // conv stage (one 4-CTA cluster per row, DMMA) + FC stage (one 8-CTA cluster, TMA-fed terr_ip0, DMMA): 2 launches instead of
-        // 15.  Plain stream order on both sides (no programmatic attribute): the pass starts after k_gather_norm has finished and the
-        // next kernel's griddepcontrol.wait covers it.
-        const int which = th == d.target ? 1 : 0;
-        FwdTrain f{};
-        f.xn = d.xn; f.rows = rows; f.S = d.S; f.cat = d.cat; f.n_out = d.n_out; f.n_frags = d.n_frags; f.frag = d.frag;
-        f.gate = pred == P_CRITIC ? &d.c->critic_ok : pred == P_CAND ? &d.c->cand_count : pred == P_ACTOR ? &d.c->actor_ok : nullptr;
-        f.a0 = keep_act ? d.a0 : nullptr; f.a1 = keep_act ? d.a1 : nullptr; f.hh = keep_act ? d.hh : nullptr;
-        f.t = d.t; f.catb = d.catb; f.h = d.h; f.y = d.y;
-        launch_forward_train(t->nw[which], t->fmaps[which], f, d.a2, st);
-        t->launches += 3;
-        return 0;
-    }
-    launch_pdl(k_conv_fwd, dim3(dim3(C0 / kConvOut, kB)), dim3(224), (size_t)kTerr * 8, st, d, pred, d.xn, d.S, 1, kTerr, blob(0), blob(1), C0, K0, d.a0);
-    launch_pdl(k_conv_fwd, dim3(dim3(C1 / kConvOut, kB)), dim3(224), (size_t)C0 * W0 * 8, st, d, pred, d.a0, C0 * W0, C0, W0, blob(2), blob(3), C1, K1, d.a1);
-    launch_pdl(k_conv_fwd, dim3(dim3(C2 / kConvOut, kB)), dim3(224), (size_t)C1 * W1 * 8, st, d, pred, d.a1, C1 * W1, C1, W1, blob(4), blob(5), C2, K2, d.a2);
-    launch_pdl(k_fc_fwd_split, dim3(dim3(T, kSplit)), dim3(256), 0, st, d, pred, d.a2, C2 * W2, C2 * W2, blob(6), T, d.part);
-    launch_pdl(k_fc_split_finish, dim3(kB), dim3(64), 0, st, d, pred, d.part, kSplit, blob(7), T, 1, d.t, T);
-    launch_pdl(k_concat, dim3(kB), dim3(160), 0, st, d, pred);
-    launch_pdl(k_fc_fwd_rows, dim3(H / 8), dim3(256), 0, st, d, pred, d.catb, d.cat, d.cat, blob(8), blob(9), H, 1, d.h, H);
-    int col = 0;
-    for (int hd = 0; hd < 4; ++hd) {
-        const int nout = hd == 0 ? d.n_frags : d.frag;
-        double* hh = d.hh + (size_t)hd * kB * HH;
-        launch_pdl(k_fc_fwd_rows, dim3(HH / 8), dim3(256), 0, st, d, pred, d.h, H, H, blob(10 + 4 * hd), blob(11 + 4 * hd), HH, 1, hh, HH);
-        launch_pdl(k_fc_fwd_rows, dim3((nout + 7) / 8), dim3(256), 0, st, d, pred, hh, HH, HH, blob(12 + 4 * hd), blob(13 + 4 * hd), nout, 0, d.y + col, d.n_out);
-        col += nout;
-    }
-    t->launches += 16;
+    // conv stage (one 4-CTA cluster per row, DMMA) + FC stage (one 8-CTA cluster, TMA-fed terr_ip0, DMMA).  Plain stream order on
+    // both sides (no programmatic attribute): the pass starts after k_gather_norm has finished and the next kernel's
+    // griddepcontrol.wait covers it.
+    const int which = net.theta == d.target ? 1 : 0;
+    FwdTrain f{};
+    f.xn = d.xn; f.rows = rows; f.S = d.S; f.cat = d.cat; f.n_out = d.n_out; f.n_frags = d.n_frags; f.frag = d.frag;
+    f.gate = pred == P_CRITIC ? &d.c->critic_ok : pred == P_CAND ? &d.c->cand_count : pred == P_ACTOR ? &d.c->actor_ok : nullptr;
+    f.a0 = keep_act ? d.a0 : nullptr; f.a1 = keep_act ? d.a1 : nullptr; f.hh = keep_act ? d.hh : nullptr;
+    f.t = d.t; f.catb = d.catb; f.h = d.h; f.y = d.y;
+    launch_forward_train(t->nw[which], t->fmaps[which], f, d.a2, st);
+    t->launches += 3;
     return 0;
 }
 // backward of the current net from d.dy (activations of the last forward) into d.grad, then the SGD step
@@ -998,56 +847,32 @@ int enqueue_backward_update(trl_trainer* t, int pred, cudaStream_t st) {
     auto W = [&](int b) { return d.theta + d.off[b]; };
     auto G = [&](int b) { return d.grad + d.off[b]; };
     const int nflat = C2 * W2;
-    if (t->fused_bwd) {
-        // 8 launches: independent bodies of one level share a launch; the four heads run side by side (dhh holds one block per head)
-        auto multi = [&](const JobList& jl) { launch_pdl(k_bwd_multi, dim3(job_blocks(jl)), dim3(256), 0, st, d, pred, jl); };
-        JobList l1{}, l2{};
-        int col = 0;
-        Job hx{}; hx.kind = J_FC_BWD_X_HEADS; hx.gx = H / 32; hx.blocks = hx.gx * kB;
-        hx.dy = d.dhh; hx.act = d.h; hx.o0 = d.dh; hx.i0 = HH; hx.i1 = HH; hx.i2 = H; hx.i3 = H; hx.i4 = H; hx.i5 = H; hx.i6 = kB * HH;
-        for (int hd = 0; hd < 4; ++hd) {
-            const int nout = hd == 0 ? d.n_frags : d.frag;
-            double* hh = d.hh + (size_t)hd * kB * HH;
-            double* dhh = d.dhh + (size_t)hd * kB * HH;
-            l1.j[l1.n++] = job_fc_w(d.dy + col, d.n_out, hh, HH, HH, nout, G(12 + 4 * hd), G(13 + 4 * hd));
-            l1.j[l1.n++] = job_fc_x(d.dy + col, d.n_out, nout, W(12 + 4 * hd), HH, HH, hh, HH, dhh, HH, 0);
-            l2.j[l2.n++] = job_fc_w(dhh, HH, d.h, H, H, HH, G(10 + 4 * hd), G(11 + 4 * hd));
-            hx.wh[hd] = W(10 + 4 * hd);
-            col += nout;
-        }
-        l2.j[l2.n++] = hx;
-        multi(l1);
-        multi(l2);
-        multi(job_list({job_fc_w(d.dh, H, d.catb, d.cat, d.cat, H, G(8), G(9)), job_fc_x(d.dh, H, H, W(8), d.cat, T, d.t, T, d.dt, T, 0)}));
-        multi(job_list({job_fc_w(d.dt, T, d.a2, nflat, nflat, T, G(6), G(7)), job_fc_x(d.dt, T, T, W(6), nflat, nflat, d.a2, nflat, d.da2, nflat, 0)}));
-        multi(job_list({job_conv_w(d.da2, C2, K2, d.a1, C1 * W1, C1, W1, G(4), G(5)), job_conv_x(d.da2, C2, K2, W(4), C1, W1, d.a1, d.da1)}));
-        multi(job_list({job_conv_w(d.da1, C1, K1, d.a0, C0 * W0, C0, W0, G(2), G(3)), job_conv_x(d.da1, C1, K1, W(2), C0, W0, d.a0, d.da0)}));
-        multi(job_list({job_conv_w(d.da0, C0, K0, d.xn, d.S, 1, kTerr, G(0), G(1))}));
-        launch_pdl(k_sgd, dim3(296), dim3(256), 0, st, d, pred);
-        t->launches += 8;
-        return 0;
-    }
+    // 8 launches: independent bodies of one level share a launch; the four heads run side by side (dhh holds one block per head)
+    auto multi = [&](const JobList& jl) { launch_pdl(k_bwd_multi, dim3(job_blocks(jl)), dim3(256), 0, st, d, pred, jl); };
+    JobList l1{}, l2{};
     int col = 0;
+    Job hx{}; hx.kind = J_FC_BWD_X_HEADS; hx.gx = H / 32; hx.blocks = hx.gx * kB;
+    hx.dy = d.dhh; hx.act = d.h; hx.o0 = d.dh; hx.i0 = HH; hx.i1 = HH; hx.i2 = H; hx.i3 = H; hx.i4 = H; hx.i5 = H; hx.i6 = kB * HH;
     for (int hd = 0; hd < 4; ++hd) {
         const int nout = hd == 0 ? d.n_frags : d.frag;
         double* hh = d.hh + (size_t)hd * kB * HH;
-        launch_pdl(k_fc_bwd_w, dim3(dim3(nout, 1)), dim3(128), 0, st, d, pred, d.dy + col, d.n_out, hh, HH, HH, G(12 + 4 * hd), G(13 + 4 * hd));
-        launch_pdl(k_fc_bwd_x, dim3(dim3(HH / 32, kB)), dim3(dim3(32, 8)), 0, st, d, pred, d.dy + col, d.n_out, nout, W(12 + 4 * hd), HH, HH, hh, HH, d.dhh, HH, 0);
-        launch_pdl(k_fc_bwd_w, dim3(dim3(HH, 1)), dim3(256), 0, st, d, pred, d.dhh, HH, d.h, H, H, G(10 + 4 * hd), G(11 + 4 * hd));
-        launch_pdl(k_fc_bwd_x, dim3(dim3(H / 32, kB)), dim3(dim3(32, 8)), 0, st, d, pred, d.dhh, HH, HH, W(10 + 4 * hd), H, H, d.h, H, d.dh, H, hd > 0);
+        double* dhh = d.dhh + (size_t)hd * kB * HH;
+        l1.j[l1.n++] = job_fc_w(d.dy + col, d.n_out, hh, HH, HH, nout, G(12 + 4 * hd), G(13 + 4 * hd));
+        l1.j[l1.n++] = job_fc_x(d.dy + col, d.n_out, nout, W(12 + 4 * hd), HH, HH, hh, HH, dhh, HH, 0);
+        l2.j[l2.n++] = job_fc_w(dhh, HH, d.h, H, H, HH, G(10 + 4 * hd), G(11 + 4 * hd));
+        hx.wh[hd] = W(10 + 4 * hd);
         col += nout;
     }
-    launch_pdl(k_fc_bwd_w, dim3(dim3(H, 1)), dim3(256), 0, st, d, pred, d.dh, H, d.catb, d.cat, d.cat, G(8), G(9));
-    launch_pdl(k_fc_bwd_x, dim3(dim3(T / 32, kB)), dim3(dim3(32, 8)), 0, st, d, pred, d.dh, H, H, W(8), d.cat, T, d.t, T, d.dt, T, 0);          // only the terr_ip0 columns
-    launch_pdl(k_fc_bwd_w, dim3(dim3(T, (nflat + 255) / 256)), dim3(256), 0, st, d, pred, d.dt, T, d.a2, nflat, nflat, G(6), G(7));
-    launch_pdl(k_fc_bwd_x, dim3(dim3((nflat + 31) / 32, kB)), dim3(dim3(32, 8)), 0, st, d, pred, d.dt, T, T, W(6), nflat, nflat, d.a2, nflat, d.da2, nflat, 0);
-    launch_pdl(k_conv_bwd_w, dim3(dim3(C1, C2)), dim3(256), 0, st, d, pred, d.da2, C2, K2, d.a1, C1 * W1, C1, W1, G(4), G(5));
-    launch_pdl(k_conv_bwd_x, dim3(dim3(C1, kB)), dim3(224), 0, st, d, pred, d.da2, C2, K2, W(4), C1, W1, d.a1, d.da1);
-    launch_pdl(k_conv_bwd_w, dim3(dim3(C0, C1)), dim3(256), 0, st, d, pred, d.da1, C1, K1, d.a0, C0 * W0, C0, W0, G(2), G(3));
-    launch_pdl(k_conv_bwd_x, dim3(dim3(C0, kB)), dim3(224), 0, st, d, pred, d.da1, C1, K1, W(2), C0, W0, d.a0, d.da0);
-    launch_pdl(k_conv_bwd_w, dim3(dim3(1, C0)), dim3(256), 0, st, d, pred, d.da0, C0, K0, d.xn, d.S, 1, kTerr, G(0), G(1));
+    l2.j[l2.n++] = hx;
+    multi(l1);
+    multi(l2);
+    multi(job_list({job_fc_w(d.dh, H, d.catb, d.cat, d.cat, H, G(8), G(9)), job_fc_x(d.dh, H, H, W(8), d.cat, T, d.t, T, d.dt, T, 0)}));
+    multi(job_list({job_fc_w(d.dt, T, d.a2, nflat, nflat, T, G(6), G(7)), job_fc_x(d.dt, T, T, W(6), nflat, nflat, d.a2, nflat, d.da2, nflat, 0)}));
+    multi(job_list({job_conv_w(d.da2, C2, K2, d.a1, C1 * W1, C1, W1, G(4), G(5)), job_conv_x(d.da2, C2, K2, W(4), C1, W1, d.a1, d.da1)}));
+    multi(job_list({job_conv_w(d.da1, C1, K1, d.a0, C0 * W0, C0, W0, G(2), G(3)), job_conv_x(d.da1, C1, K1, W(2), C0, W0, d.a0, d.da0)}));
+    multi(job_list({job_conv_w(d.da0, C0, K0, d.xn, d.S, 1, kTerr, G(0), G(1))}));
     launch_pdl(k_sgd, dim3(296), dim3(256), 0, st, d, pred);
-    t->launches += 26;
+    t->launches += 8;
     return 0;
 }
 // cNeuralNetTrainer::Train: UpdateStage, then num_steps_per_iter x cMACETrainer::Step, then IncIter
@@ -1066,26 +891,15 @@ int enqueue_train(trl_trainer* t, cudaStream_t st) {
         // -- the critic's s', the actor candidates' s and s' -- goes through it in ONE pass of 3 kB rows (three FC clusters side by side)
         launch_pdl(k_sample_critic, dim3(1), dim3(32), 0, st, d);
         launch_pdl(k_sample_actor, dim3(1), dim3(32), 0, st, d);
-        if (t->batched_fwd) {
-            enqueue_forward(t, P_ALWAYS, col_end, tar, st, false, col_beg, col_end, 0x6);
-        } else {
-            enqueue_forward(t, P_CRITIC, col_end, tar, st, false);
-        }
+        enqueue_forward(t, P_ALWAYS, col_end, tar, st, false, col_beg, col_end, 0x6);
         // ---- critic: BuildProblem + UpdateNet (learning/NeuralNetTrainer.cpp:414-456, MACETrainer.cpp:222-247)
         launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CRITIC, 1, d.v1, 0, 0);
         enqueue_forward(t, P_CRITIC, col_beg, cur, st);
         launch_pdl(k_labels, dim3(1), dim3(256), 0, st, d, P_CRITIC, 0);
         enqueue_backward_update(t, P_CRITIC, st);
         // ---- actor: UpdateActorBatchBuffer + UpdateActor (learning/MACETrainer.cpp:541-626)
-        if (t->batched_fwd) {
-            launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 0, d.v0, kB, 1);
-            launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 1, d.v1, 2 * kB, 1);
-        } else {
-            enqueue_forward(t, P_CAND, col_beg, tar, st, false, -1, -1, 0x1);
-            launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 0, d.v0, 0, 1);
-            enqueue_forward(t, P_CAND, col_end, tar, st, false, -1, -1, 0x1);
-            launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 1, d.v1, 0, 1);
-        }
+        launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 0, d.v0, kB, 1);
+        launch_pdl(k_vals, dim3(1), dim3(32), 0, st, d, P_CAND, 1, d.v1, 2 * kB, 1);
         launch_pdl(k_actor_select, dim3(1), dim3(32), 0, st, d);
         enqueue_forward(t, P_ACTOR, col_beg, cur, st);
         launch_pdl(k_labels, dim3(1), dim3(256), 0, st, d, P_ACTOR, 1);
@@ -1172,12 +986,11 @@ trl_trainer* trl_trainer_create(trl_handle* h, const double* p) {
     A(talloc(t, &d.h, (size_t)3 * kB * H)); A(talloc(t, &d.hh, (size_t)4 * kB * HH)); A(talloc(t, &d.y, (size_t)3 * kB * d.n_out));
     A(talloc(t, &d.v0, kB)); A(talloc(t, &d.v1, kB)); A(talloc(t, &d.dy, (size_t)kB * d.n_out)); A(talloc(t, &d.dhh, (size_t)4 * kB * HH));
     A(talloc(t, &d.dh, (size_t)kB * H)); A(talloc(t, &d.dt, (size_t)kB * T)); A(talloc(t, &d.da2, (size_t)kB * C2 * W2));
-    A(talloc(t, &d.da1, (size_t)kB * C1 * W1)); A(talloc(t, &d.da0, (size_t)kB * C0 * W0)); A(talloc(t, &d.mean, d.S)); A(talloc(t, &d.part, (size_t)kSplit * kB * T));
+    A(talloc(t, &d.da1, (size_t)kB * C1 * W1)); A(talloc(t, &d.da0, (size_t)kB * C0 * W0)); A(talloc(t, &d.mean, d.S));
     t->stage_cap = add_cap;
     t->gather_cap = add_cap;
     A(talloc(t, &t->stage_rows, (size_t)add_cap * d.Wd)); A(talloc(t, &t->stage_flags, add_cap));
     if (ok) {
-        A(cudaFuncSetAttribute(k_conv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, C1 * W1 * 8));
         A(cudaMemset(d.pos_critic, 0xff, (size_t)d.cap * 4));
         A(cudaMemset(d.pos_actor, 0xff, (size_t)d.cap * 4));
         cudaStreamSynchronize(h->stream);
@@ -1192,33 +1005,18 @@ trl_trainer* trl_trainer_create(trl_handle* h, const double* p) {
         delete t;
         return nullptr;
     }
-    {
-        const char* v1 = std::getenv("TRL_TRAIN_FWD_V1");
-        t->batched_fwd = !(v1 && v1[0] == '1');
-        const char* b1 = std::getenv("TRL_TRAIN_BWD_V1");
-        t->fused_bwd = !(b1 && b1[0] == '1');
-        const double* bases[2] = {d.theta, d.target};
-        for (int k = 0; k < 2 && t->batched_fwd; ++k) {
-            NetWeights& W = t->nw[k];
-            auto bl = [&](int b) { return (const double*)(bases[k] + d.off[b]); };
-            W.conv0_w = bl(0); W.conv0_b = bl(1); W.conv1_w = bl(2); W.conv1_b = bl(3); W.conv2_w = bl(4); W.conv2_b = bl(5);
-            W.tip0_w = bl(6); W.tip0_b = bl(7); W.ip0_w = bl(8); W.ip0_b = bl(9);
-            for (int q = 0; q < 4; ++q) { W.h0_w[q] = bl(10 + 4 * q); W.h0_b[q] = bl(11 + 4 * q); W.h1_w[q] = bl(12 + 4 * q); W.h1_b[q] = bl(13 + 4 * q); }
-            W.in_off = W.in_scale = W.out_off = W.out_scale = nullptr;          // the minibatch arrives normalised; outputs stay normalised
-            if (trl_make_fc_maps(&t->fmaps[k], W.tip0_w, d.a2, 3 * kB)) {
-                for (void* q : t->allocs) cudaFree(q);
-                delete t;
-                return nullptr;
-            }
+    const double* blobs[2][26];            // the blobs of the current net (in theta) and of the target net (in target)
+    for (int b = 0; b < 26; ++b) { blobs[0][b] = d.theta + d.off[b]; blobs[1][b] = d.target + d.off[b]; }
+    for (int k = 0; k < 2; ++k) {
+        t->nw[k] = net_weights(blobs[k], nullptr, nullptr, nullptr, nullptr);     // the minibatch arrives normalised; outputs stay normalised
+        if (trl_make_fc_maps(&t->fmaps[k], t->nw[k].tip0_w, d.a2, 3 * kB)) {
+            for (void* q : t->allocs) cudaFree(q);
+            delete t;
+            return nullptr;
         }
     }
     // cNeuralNetLearner::SyncNet as a binding: the decision kernel reads the trainer's weights from now on
-    NetWeights& Wt = h->W;
-    auto blob = [&](int b) { return (const double*)(d.theta + d.off[b]); };
-    Wt.conv0_w = blob(0); Wt.conv0_b = blob(1); Wt.conv1_w = blob(2); Wt.conv1_b = blob(3); Wt.conv2_w = blob(4); Wt.conv2_b = blob(5);
-    Wt.tip0_w = blob(6); Wt.tip0_b = blob(7); Wt.ip0_w = blob(8); Wt.ip0_b = blob(9);
-    for (int k = 0; k < 4; ++k) { Wt.h0_w[k] = blob(10 + 4 * k); Wt.h0_b[k] = blob(11 + 4 * k); Wt.h1_w[k] = blob(12 + 4 * k); Wt.h1_b[k] = blob(13 + 4 * k); }
-    Wt.in_off = d.in_off; Wt.in_scale = d.in_scale; Wt.out_off = d.out_off; Wt.out_scale = d.out_scale;
+    h->W = net_weights(blobs[0], d.in_off, d.in_scale, d.out_off, d.out_scale);
     trl_drop_graphs(h);
     h->trainer = t;
     return t;
@@ -1256,12 +1054,8 @@ int trl_trainer_destroy(trl_trainer* t) {
     for (int b = 0; b < 26; ++b) cudaMemcpy(h->net_blobs[b], t->d.theta + t->d.off[b], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice);
     cudaMemcpy(h->net_blobs[26], t->d.in_off, (size_t)h->net_counts[26] * 8, cudaMemcpyDeviceToDevice);
     cudaMemcpy(h->net_blobs[27], t->d.in_scale, (size_t)h->net_counts[27] * 8, cudaMemcpyDeviceToDevice);
-    NetWeights& W = h->W;
     double** b = h->net_blobs.data();
-    W.conv0_w = b[0]; W.conv0_b = b[1]; W.conv1_w = b[2]; W.conv1_b = b[3]; W.conv2_w = b[4]; W.conv2_b = b[5];
-    W.tip0_w = b[6]; W.tip0_b = b[7]; W.ip0_w = b[8]; W.ip0_b = b[9];
-    for (int k = 0; k < 4; ++k) { W.h0_w[k] = b[10 + 4 * k]; W.h0_b[k] = b[11 + 4 * k]; W.h1_w[k] = b[12 + 4 * k]; W.h1_b[k] = b[13 + 4 * k]; }
-    W.in_off = b[26]; W.in_scale = b[27]; W.out_off = b[28]; W.out_scale = b[29];
+    h->W = net_weights(b, b[26], b[27], b[28], b[29]);
     trl_drop_graphs(h);
     h->trainer = nullptr;
     if (t->train_graph) cudaGraphExecDestroy(t->train_graph);
@@ -1364,12 +1158,12 @@ int trl_trainer_train(trl_trainer* t, int iters) {
         TCK(cudaStreamEndCapture(t->work(), &graph));
         TCK(cudaGraphInstantiate(&t->train_graph, graph, 0));
         cudaGraphDestroy(graph);
+        t->graph_launches = t->launches - before;      // capturing ran no kernel; each replay runs the kernels it recorded
         t->launches = before;
     }
-    const int per = 5 + t->d.steps_per_iter * (10 + (t->batched_fwd ? 3 * 3 : 5 * 16) + 2 * (t->fused_bwd ? 8 : 26));
     for (int i = 0; i < iters; ++i) {
         TCK(cudaGraphLaunch(t->train_graph, t->work()));
-        t->launches += per;
+        t->launches += t->graph_launches;
     }
     return 0;
 }
@@ -1438,14 +1232,13 @@ int trl_trainer_set_async(trl_trainer* t, int enable) {
     TCK(trainer_sync(t));
     const Dev& d = t->d;
     if (t->train_graph) { cudaGraphExecDestroy(t->train_graph); t->train_graph = nullptr; }      // it was captured on the other stream
-    NetWeights& W = h->W;
     if (enable) {
         if (!h->comm) return trl_fail("trl_trainer_set_async: asynchronous training needs a communicator (trl_comm_init first)");
         if (!t->async_stream) {
             int lo = 0, hi = 0;
             cudaDeviceGetStreamPriorityRange(&lo, &hi);
-            // highest priority: the trainer's ~140 launches per iteration are a few CTAs each; behind the step launch's CTAs every
-            // one of them would wait for a free slot
+            // highest priority: the trainer's launches are a few CTAs each; behind the step launch's CTAs every one of them would
+            // wait for a free slot
             TCK(cudaStreamCreateWithPriority(&t->async_stream, cudaStreamNonBlocking, hi));
             TCK(cudaEventCreateWithFlags(&t->ev_snap, cudaEventDisableTiming));
             TCK(cudaEventCreateWithFlags(&t->ev_trained, cudaEventDisableTiming));
@@ -1460,14 +1253,10 @@ int trl_trainer_set_async(trl_trainer* t, int enable) {
     }
     // bind the decision kernels to the snapshot (async) or straight to the trainer's arrays (synchronous: SyncNet as a pointer binding)
     const double* th = enable ? t->snap : d.theta;
-    auto blob = [&](int b) { return th + d.off[b]; };
-    W.conv0_w = blob(0); W.conv0_b = blob(1); W.conv1_w = blob(2); W.conv1_b = blob(3); W.conv2_w = blob(4); W.conv2_b = blob(5);
-    W.tip0_w = blob(6); W.tip0_b = blob(7); W.ip0_w = blob(8); W.ip0_b = blob(9);
-    for (int k = 0; k < 4; ++k) { W.h0_w[k] = blob(10 + 4 * k); W.h0_b[k] = blob(11 + 4 * k); W.h1_w[k] = blob(12 + 4 * k); W.h1_b[k] = blob(13 + 4 * k); }
-    W.in_off = enable ? t->snap + d.P : d.in_off;
-    W.in_scale = enable ? t->snap + d.P + d.S : d.in_scale;
-    W.out_off = enable ? t->snap + d.P + 2 * d.S : d.out_off;
-    W.out_scale = enable ? t->snap + d.P + 2 * d.S + d.n_out : d.out_scale;
+    const double* blobs[26];
+    for (int b = 0; b < 26; ++b) blobs[b] = th + d.off[b];
+    h->W = net_weights(blobs, enable ? t->snap + d.P : d.in_off, enable ? t->snap + d.P + d.S : d.in_scale,
+                       enable ? t->snap + d.P + 2 * d.S : d.out_off, enable ? t->snap + d.P + 2 * d.S + d.n_out : d.out_scale);
     trl_drop_graphs(h);
     t->async = enable != 0;
     t->trained_pending = t->job_pending = false;

@@ -156,6 +156,17 @@ struct NetWeights {
     const double *h0_w[4], *h0_b[4], *h1_w[4], *h1_b[4];
     const double *in_off, *in_scale, *out_off, *out_scale;
 };
+// Binds the 26 weight blobs (w, b per layer: terr_conv0..2, terr_ip0, ip0, then h0 w, h0 b, h1 w, h1 b of each of the four heads)
+// and the input / output offset and scale vectors.  The vectors may be null for a net that is fed normalised inputs.
+inline NetWeights net_weights(const double* const* b, const double* in_off, const double* in_scale, const double* out_off,
+                              const double* out_scale) {
+    NetWeights W;
+    W.conv0_w = b[0]; W.conv0_b = b[1]; W.conv1_w = b[2]; W.conv1_b = b[3]; W.conv2_w = b[4]; W.conv2_b = b[5];
+    W.tip0_w = b[6]; W.tip0_b = b[7]; W.ip0_w = b[8]; W.ip0_b = b[9];
+    for (int k = 0; k < 4; ++k) { W.h0_w[k] = b[10 + 4 * k]; W.h0_b[k] = b[11 + 4 * k]; W.h1_w[k] = b[12 + 4 * k]; W.h1_b[k] = b[13 + 4 * k]; }
+    W.in_off = in_off; W.in_scale = in_scale; W.out_off = out_off; W.out_scale = out_scale;
+    return W;
+}
 
 // Device buffers of one batch of environments.
 struct Buffers {

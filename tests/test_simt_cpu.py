@@ -259,7 +259,7 @@ def test_env_groups_match_the_monolithic_launch(assets, monkeypatch):
             sc.close()
 
 
-def test_trainer_kernels_vs_oracle(assets, monkeypatch):
+def test_trainer_kernels_vs_oracle(assets):
     from pyoracle import OracleTrainer
     from test_gpu_trainer import _synthetic_tuples
     import deepterrainrl_b200 as trl
@@ -268,22 +268,14 @@ def test_trainer_kernels_vs_oracle(assets, monkeypatch):
     with simt_library():
         sc = trl.ScenarioExpMACE(pack, 4)
         g = trl.MACETrainer(sc, replay_mem_size=160, **kw)
-        # the same trainer with one launch per backward kernel (26 per pass) instead of the 8 multi-body launches: bit-identical weights
-        monkeypatch.setenv("TRL_TRAIN_BWD_V1", "1")
-        sc1 = trl.ScenarioExpMACE(pack, 4)
-        g1 = trl.MACETrainer(sc1, replay_mem_size=160, **kw)
-        monkeypatch.delenv("TRL_TRAIN_BWD_V1")
         o = OracleTrainer(pack, replay_cap=160, **kw)
         rows, flags = _synthetic_tuples(128, g.S, g.A, o.get("in_off"), o.get("in_scale"), 3)
         g.AddTuples(rows, flags)
-        g1.AddTuples(rows, flags)
         o.add_tuples(rows, flags)
         for it in range(2):   # the second iteration includes an actor step
-            l0, l1 = g.KernelLaunches(), g1.KernelLaunches()
+            l0 = g.KernelLaunches()
             g.Train(1)
-            g1.Train(1)
-            assert (g.KernelLaunches() - l0, g1.KernelLaunches() - l1) == (40, 76)
-            np.testing.assert_array_equal(g.get("theta"), g1.get("theta"))
+            assert g.KernelLaunches() - l0 == 40
             o.train()
             cg, co = g.counters(), o.counters()
             for k in ("iter", "actor_iter", "stage", "num", "head", "total", "critic", "actor", "actor_batch"):
@@ -322,11 +314,10 @@ def test_trainer_kernels_vs_oracle(assets, monkeypatch):
         with pytest.raises(RuntimeError, match="has been destroyed"):
             g.Train(1)
         g.close()
-        g1.close(); sc1.close()
 
 
 def test_trainer_kernels_have_no_schedule_dependent_results(assets):
-    """The trainer's ~140 launches per iteration lean on __syncthreads and shared-memory staging: same race check as for the
+    """The trainer's kernels lean on __syncthreads and shared-memory staging: same race check as for the
     step / decision kernels -- a permuted thread schedule must not change a single weight."""
     from test_gpu_trainer import _synthetic_tuples
     import deepterrainrl_b200 as trl
