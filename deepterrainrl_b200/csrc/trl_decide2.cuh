@@ -18,7 +18,8 @@
 //                            then the scalar decision logic of cDogControllerMACE::UpdateAction / cBaseControllerMACE::
 //                            DecideActionBoltzmann for up to 32 decisions at once, one lane each.
 //
-// Results differ from trl_decide.cuh's single-decision pass only in summation order (<= 1e-13 relative on the net outputs).
+// Results differ from trl_decide.cuh's single-decision pass only in summation order (<= 1e-13 relative on the net outputs;
+// tests/test_gpu_decide_batches.py checks this and the batch shapes the FC stage branches on).
 #pragma once
 #include <cooperative_groups.h>
 

@@ -1276,20 +1276,70 @@ int trl_get_terrain(trl_handle* h, int env, int seg, float* data, int cap, int* 
 
 int64_t trl_kernel_launches(trl_handle* h) { return h ? h->launches : -1; }
 
+// Stage pending list 0 for the debug entry points below: `env_ids` (NULL = envs 0 .. n-1) with count n, on the handle's stream.
+// The decision launch that consumes the list with rearm = 1 resets the count, so this runs before every launch.
+static int stage_pending_list(trl_handle* h, const int32_t* env_ids, int n) {
+    std::vector<int32_t> ids;
+    if (!env_ids) {
+        ids.resize(n);
+        for (int i = 0; i < n; ++i) ids[i] = i;
+        env_ids = ids.data();
+    }
+    if (n > 0) CK(cudaMemcpyAsync(h->B.pending_list, env_ids, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->B.pending_count, &n, 4, cudaMemcpyHostToDevice, h->stream));
+    return 0;
+}
+
+// One decision pass over a chosen batch (tests): the listed envs, in list order (row k of the pass = env_ids[k]), optionally with
+// new policy states, through the same launch(es) one env-step's decisions take.  Returns after the pass has finished.
+int trl_debug_decide(trl_handle* h, const int32_t* env_ids, int n, const double* poli_states) {
+    if (!h) return fail("trl_debug_decide: null handle");
+    if (n < 0 || n > h->n) return fail("trl_debug_decide: env count out of range");
+    if (n > 0 && !env_ids) return fail("trl_debug_decide: no env list");
+    {
+        std::vector<char> seen(h->n, 0);
+        for (int k = 0; k < n; ++k) {
+            const int e = env_ids[k];
+            if (e < 0 || e >= h->n) return fail("trl_debug_decide: env id out of range");
+            if (seen[e]) return fail("trl_debug_decide: env " + std::to_string(e) + " listed twice");
+            seen[e] = 1;
+        }
+    }
+    if (ensure_model(h)) return fail("model upload failed");
+    // idle handle: the overlapped schedule leaves decisions and catch-up launches on the side streams and env groups on theirs
+    CK(cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < h->lag; ++k) CK(cudaStreamSynchronize(h->side[k]));
+    for (int g = 0; g < kMaxGroups - 1; ++g)
+        if (h->group_stream[g]) CK(cudaStreamSynchronize(h->group_stream[g]));
+    if (poli_states) {
+        const size_t S = (size_t)h->B.S;
+        for (int k = 0; k < n;) {      // one copy per run of consecutive env ids
+            int r = 1;
+            while (k + r < n && env_ids[k + r] == env_ids[k] + r) ++r;
+            CK(cudaMemcpyAsync(h->B.poli_state + (size_t)env_ids[k] * S, poli_states + (size_t)k * S, (size_t)r * S * 8, cudaMemcpyHostToDevice,
+                               h->stream));
+            k += r;
+        }
+    }
+    if (stage_pending_list(h, env_ids, n)) return 1;
+    enqueue_decide(h, 0, 1, h->stream);
+    h->launches += num_decide_launches(h);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
 // Micro-benchmark of the decision kernel: marks the first `n_pending` envs as pending (their policy state is whatever the
 // last real decision left) and times `iters` launches.  Perturbs those envs' actions: measurement use only.
 int trl_debug_time_decide(trl_handle* h, int n_pending, int iters, double* ms_avg) {
     if (!h) return fail("trl_debug_time_decide: null handle");
     if (ensure_model(h)) return fail("model upload failed");
     if (n_pending > h->n) n_pending = h->n;
-    std::vector<int> ids(n_pending);
-    for (int i = 0; i < n_pending; ++i) ids[i] = i;
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
     double total = 0;
     for (int it = 0; it < iters; ++it) {
-        CK(cudaMemcpyAsync(h->B.pending_list, ids.data(), (size_t)n_pending * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->B.pending_count, &n_pending, 4, cudaMemcpyHostToDevice, h->stream));
+        if (stage_pending_list(h, nullptr, n_pending)) return 1;
         CK(cudaEventRecord(e0, h->stream));
         enqueue_decide(h, 0, 1, h->stream);
         CK(cudaEventRecord(e1, h->stream));
@@ -1310,8 +1360,6 @@ int trl_debug_fc_phases(trl_handle* h, int n_pending, double* out_ns16, double* 
     if (!h->decide_v2 || !h->mc.has_net) return fail("trl_debug_fc_phases: the batched decision path is not active");
     if (ensure_model(h)) return fail("model upload failed");
     n_pending = std::max(1, std::min(n_pending, h->n));
-    std::vector<int> ids(n_pending);
-    for (int i = 0; i < n_pending; ++i) ids[i] = i;
     unsigned long long* prof = nullptr;
     CK(cudaMalloc((void**)&prof, 16 * 8));
     CK(cudaMemset(prof, 0, 16 * 8));
@@ -1320,8 +1368,7 @@ int trl_debug_fc_phases(trl_handle* h, int n_pending, double* out_ns16, double* 
     cudaEvent_t e0, e1, e2;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
     for (int it = 0; it < 3; ++it) {      // the last of three runs is reported (weights L2-resident, clocks up)
-        CK(cudaMemcpyAsync(h->B.pending_list, ids.data(), (size_t)n_pending * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->B.pending_count, &n_pending, 4, cudaMemcpyHostToDevice, h->stream));
+        if (stage_pending_list(h, nullptr, n_pending)) return 1;
         CK(cudaEventRecord(e0, h->stream));
         launch_decide2(h->B, h->W, h->d_ex, maps, h->act2[0], h->done_count, h->decide_grid, h->fc_clusters, 0, 1, h->stream, 1);
         CK(cudaEventRecord(e1, h->stream));

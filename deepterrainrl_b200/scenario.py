@@ -122,7 +122,7 @@ EXPORTS = [
     "trl_set_explore", "trl_set_phys_params", "trl_set_weights", "trl_sizes", "trl_num_tuples", "trl_get_tuples",
     "trl_get_tuples_f64", "trl_reset_tuples", "trl_eval_stats", "trl_dist_log", "trl_reset_avg_dist", "trl_get_state", "trl_set_state",
     "trl_get_state_all", "trl_get_ctrl", "trl_get_poli_state", "trl_get_net_out", "trl_get_layer_state", "trl_get_terrain",
-    "trl_kernel_launches", "trl_last_error", "trl_bench_updates", "trl_update_timed", "trl_device_tuple_block", "trl_snapshot", "trl_snapshot_wait", "trl_update_timed_detail", "trl_update_timeline", "trl_debug_time_decide", "trl_debug_fc_phases", "trl_debug_step_phases",
+    "trl_kernel_launches", "trl_last_error", "trl_bench_updates", "trl_update_timed", "trl_device_tuple_block", "trl_snapshot", "trl_snapshot_wait", "trl_update_timed_detail", "trl_update_timeline", "trl_debug_time_decide", "trl_debug_decide", "trl_debug_fc_phases", "trl_debug_step_phases",
     "trl_load_model", "trl_output_model", "trl_write_model", "trl_get_output_offset_scale", "trl_pack_output_offset_scale",
     "trl_set_terrain_lerp", "trl_train_schedule", "trl_trainer_create", "trl_trainer_destroy", "trl_trainer_init_fresh", "trl_trainer_add_from_scene", "trl_trainer_add_tuples", "trl_trainer_add_device", "trl_trainer_train", "trl_train_run", "trl_train_run_timed",
     "trl_trainer_counters", "trl_trainer_num_params", "trl_trainer_launches", "trl_trainer_get", "trl_trainer_set_theta", "trl_trainer_list", "trl_trainer_rows",
@@ -285,6 +285,13 @@ class BatchedScenario:
         y = np.zeros(96)
         self._ck(self.L.trl_get_net_out(self.h, env, _p(y)))
         return y[:n]
+
+    def DebugDecide(self, env_ids, poli_states=None):
+        """tests: one decision pass over exactly these envs (row k = env_ids[k]), after writing poli_states ([n, state_size]) into
+        their policy states if given"""
+        ids = np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        x = None if poli_states is None else np.ascontiguousarray(poli_states, dtype=np.float64).reshape(ids.size, self.state_size)
+        self._ck(self.L.trl_debug_decide(self.h, _p(ids), int(ids.size), _p(x)))
 
     def GetLayerState(self, layer_name, env=0):
         """cNeuralNet::GetLayerState: the named blob of the deploy net for the policy state of env's last decision"""

@@ -126,6 +126,10 @@ int trl_update_timed_detail(trl_handle* h, double dt, double* per_step_ms, doubl
 int trl_update_timeline(trl_handle* h, double dt, double* out4, int cap, int* n);
 
 int trl_debug_time_decide(trl_handle* h, int n_pending, int iters, double* ms_avg);
+/* tests: one policy decision pass over the listed envs, row k = env_ids[k] (distinct ids, 0 <= n <= num_envs; n = 0 changes nothing).
+ * poli_states: NULL, or [n][state] rows written into those envs' policy states first.  Waits for the handle's queued work, runs the
+ * decision launch(es) of one env-step on that list and returns when they have finished. */
+int trl_debug_decide(trl_handle* h, const int32_t* env_ids, int n, const double* poli_states);
 /* measurement only: in-kernel phase stamps (ns from entry, 16 slots) of the batched decision path's FC kernel + event-timed conv / FC launches */
 int trl_debug_fc_phases(trl_handle* h, int n_pending, double* out_ns16, double* conv_us, double* fc_us);
 /* measurement only, TRL_PHASE_CLOCKS=1 builds: clock64() cycles of the env-step kernel summed over warps per phase (9 slots: state

@@ -437,6 +437,36 @@ def test_experimental_variant_is_bit_identical(assets, defines, scene, variant_b
         assert np.array_equal(ref, _trajectory(defines, pack, 3, 130, seed=99, updates=1))
 
 
+def test_decision_batches_vs_torch(assets):
+    """The batched decision pass on chosen env lists (trl_debug_decide), the sweep of tests/test_gpu_decide_batches.py in miniature:
+    70 envs, so 2 FC clusters x 32-row chunks and (4 emulated SMs) 2 conv clusters.  67 decisions = a second chunk on cluster 0, ragged,
+    running past row 70 of act2 into the zero fill; permuted / reversed / tail / strided lists.  Outputs vs torch f64, the committed
+    action vs torch's arg-max, every other env untouched, an env's output bit-identical alone and at rows 0 / 66.  The emulator copies
+    the tiles TMA would load, so this pins the row / env / chunk indexing, not the TMA ring (that is the GPU test's part)."""
+    import torch_net
+    from pack_scene import read_pack
+    from test_gpu_decide_batches import StatePool, assert_unchanged, batch_invariance, decide_and_check, edge_states, env_ids, \
+        refuses_bad_lists, snapshot
+    import deepterrainrl_b200 as trl
+    pack = os.path.join(assets, "dog_slopes_mixed.trlpack")
+    net = torch_net.blobs_from_pack(read_pack(pack))
+    recorded = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "first_decision.npz"))["poli_state"]
+    n = 70
+    pool = StatePool(net, n, np.concatenate([recorded[None], edge_states(net[1], net[2], 2, 3)]), seed=1)
+    with simt_library():
+        sc = trl.ScenarioPoliEval(pack, n)
+        worst = decide_and_check(sc, pool, env_ids("identity", n, n), 90, watch=[])
+        for order, count in (("permuted", 67), ("reversed", 65), ("last", 33), ("strided", 5)):
+            worst = max(worst, decide_and_check(sc, pool, env_ids(order, count, n, seed=1), 90))
+        assert worst <= 1e-10, worst
+        before = snapshot(sc, range(n), 90)
+        sc.DebugDecide([])
+        assert_unchanged(sc, before, 90, 0)
+        batch_invariance(sc, pool, [4], [0, 66], 67, 90)
+        refuses_bad_lists(sc)
+        sc.close()
+
+
 def test_layer_state_probe_vs_oracle(assets):
     """trl_get_layer_state (csrc/trl_probe.cu; cNeuralNet::GetLayerState behind RecordNNActivation) on the emulator against the oracle's
     blobs (oracle/net.h: layer_state, itself checked against torch in tests/test_net_torch_cpu.py) for every top of the deploy net"""
