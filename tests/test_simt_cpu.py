@@ -134,6 +134,38 @@ def test_kernel_sources_reproduce_the_compiled_reference(assets, scene):
         sc.close()
 
 
+@pytest.mark.parametrize("scene,vertex", [("dog_slopes_mixed", False), ("raptor_narrow_gaps", False), ("goat_cliffs", True)])
+def test_forced_steps_and_stress_states_vs_oracle(assets, monkeypatch, scene, vertex):
+    """tests/test_gpu_step_forced.py in miniature: 3 envs, 40 forced env-steps (each from the oracle's state), then one instance
+    of every stress kind (two of friction: below and above v_eps), 5 forced steps each.  Without FMA contraction q, the
+    controller block, the policy state and the net output agree to 1e-12.  qd and the held torque come out of the two
+    different solves (articulated-body passes here, CRBA + LDL^T in the oracle): the oracle itself moves them by 1e-12 .. 4e-12
+    when its input state is perturbed by 1e-15 relative, so they are held to 5e-11, and q, which integrates qd over the step,
+    to 5e-12; a stiff stress state, where 100x that sensitivity is larger, is held to that instead (F.Sensitivity).  The goat runs the vertex contact model
+    (TRL_VERTEX_CONTACTS=1 / ORC_VTX=1), with two more states that put a convex terrain vertex into a box.
+
+    Planted one at a time in trl_step.cu, each of these makes this test fail (and each also fails some older test of this file):
+    the dt * cl joint-limit armature dropped from the chain pass (all three cases; qd off by 1e-2 .. 2), the touching test
+    pen > -contact_tol changed to pen > 0 (all three; contact bits differ), kClearMargin = 0 (raptor and goat; a contact bit of
+    a corner in the touching band above the window maximum differs), ci & 3 changed to ci & 1 in the vertex rounds (goat; qd
+    off by 0.36)."""
+    import test_gpu_step_forced as F
+    n = 3
+    kinds = F.KINDS + ("friction",) + (("vertex", "vertex") if vertex else ())
+    if vertex:
+        monkeypatch.setenv("TRL_VERTEX_CONTACTS", "1")
+        monkeypatch.setenv("ORC_VTX", "1")
+    with simt_library():
+        g, o, m = F.make_pair(assets, scene, n)
+        sens = F.Sensitivity(assets, scene, n)
+        worst = F.Worst({"default": 1e-12, "q": 5e-12, "qd": 5e-11, "tau": 5e-11})
+        F.forced_steps(g, o, m, range(n), 40, worst, scene, sens=sens)
+        cov = F.stress_rounds(g, o, m, n, 4 if vertex else 3, worst, scene, seed=11, kinds=kinds, sens=sens)
+        g.close()
+    worst.report()
+    cov.check(scene, kinds)
+
+
 def test_update_graph_overlapped_schedule_and_tuples_vs_oracle(assets):
     """trl_update: captured graph, two-stream schedule with catch-up launches, exploration on; tuples and counters."""
     n = 4
