@@ -264,39 +264,24 @@ static int fill_model(trl_handle* h, uint64_t rng_seed) {
         for (int k = 1; k < 4; ++k) m.anc_pow[j][k] = m.anc_pow[j][k - 1] >= 0 ? m.anc_pow[m.anc_pow[j][k - 1]][k - 1] : -1;
     }
     {
-        // box corners, ordered so that the bodies most likely to touch the ground (lowest in the zero pose: feet, shanks)
-        // share the first 32-corner round; rounds whose corners are all clear of the terrain are skipped by the kernel.
+        // box corners in the link frame, the 4 of a collidable body from corner_base[j] on (the body's lane tests them in this order).
         // reach = upper bound of |corner - root joint| over all poses (bounds the terrain window the contacts can see)
-        std::vector<double> jy(m.nj, 0.0), jr(m.nj, 0.0), low(m.nj, 0.0);
-        std::vector<int> order;
+        std::vector<double> jr(m.nj, 0.0);
         m.reach = 0.0;
+        m.n_corners = 0;
         for (int j = 0; j < m.nj; ++j) {
-            if (j > 0) {
-                jy[j] = jy[m.parent[j]] + m.attach_y[j];
-                jr[j] = jr[m.parent[j]] + std::hypot(m.attach_x[j], m.attach_y[j]);
-            }
+            if (j > 0) jr[j] = jr[m.parent[j]] + std::hypot(m.attach_x[j], m.attach_y[j]);
             m.corner_base[j] = -1;
             if (!m.collidable[j]) continue;
-            order.push_back(j);
-            low[j] = 1e30;
+            m.corner_base[j] = m.n_corners;
             for (int cn = 0; cn < 4; ++cn) {
                 double bx = (cn & 1) ? m.half_x[j] : -m.half_x[j], by = (cn & 2) ? m.half_y[j] : -m.half_y[j];
                 double lx = m.body_ax[j] + m.body_cos[j] * bx - m.body_sin[j] * by;
                 double ly = m.body_ay[j] + m.body_sin[j] * bx + m.body_cos[j] * by;
-                low[j] = std::min(low[j], jy[j] + ly);
-                m.reach = std::max(m.reach, jr[j] + std::hypot(lx, ly));
-            }
-        }
-        std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return low[a] < low[b]; });
-        m.n_corners = 0;
-        for (int j : order) {
-            m.corner_base[j] = m.n_corners;
-            for (int cn = 0; cn < 4; ++cn) {
-                double bx = (cn & 1) ? m.half_x[j] : -m.half_x[j], by = (cn & 2) ? m.half_y[j] : -m.half_y[j];
-                m.corner_body[m.n_corners] = j;
-                m.corner_lx[m.n_corners] = m.body_ax[j] + m.body_cos[j] * bx - m.body_sin[j] * by;
-                m.corner_ly[m.n_corners] = m.body_ay[j] + m.body_sin[j] * bx + m.body_cos[j] * by;
+                m.corner_lx[m.n_corners] = lx;
+                m.corner_ly[m.n_corners] = ly;
                 ++m.n_corners;
+                m.reach = std::max(m.reach, jr[j] + std::hypot(lx, ly));
             }
         }
     }

@@ -104,7 +104,8 @@ constexpr int X_CHO_END = X_CHO + kMaxJoints * kChainStride;
 // stores / loads); values and operation order are untouched, so every variant is bit-identical to the default build
 // (tests/test_simt_cpu.py checks that on the CPU emulator).  Default build: all off.  -DTRL_SMEM_XCHG=1: all on.
 // TRL_ACCUM_SMEM and TRL_LDLT_SMEM name exchanges the chain passes removed (the round-by-round child -> parent hand-off, the
-// LDL^T pivot column); they are accepted and change nothing.
+// LDL^T pivot column), TRL_CONTACT_SMEM the corner -> body-lane exchanges the per-body contact pass removed; they are accepted and
+// change nothing.
 #ifndef TRL_SMEM_XCHG
 #define TRL_SMEM_XCHG 0
 #endif
@@ -114,21 +115,11 @@ constexpr int X_CHO_END = X_CHO + kMaxJoints * kChainStride;
 #ifndef TRL_OUTWARD_SMEM
 #define TRL_OUTWARD_SMEM TRL_SMEM_XCHG   // floating-base broadcast of the root's articulated inertia (9 doubles x 6 per env-step)
 #endif
-#ifndef TRL_CONTACT_SMEM
-#define TRL_CONTACT_SMEM TRL_SMEM_XCHG   // corner lanes read their body's kinematics, owners collect contact forces (7-21 + 9 per contact, x 5)
-#endif
-#if TRL_CONTACT_SMEM
-constexpr int kAccStride = 10;                              // doubles per lane slot: 9 values, padded to 80 B (128-bit accesses stay conflict-free)
-constexpr int X_ACC = X_CHO_END;
-constexpr int X_ACC_END = X_ACC + kWarp * kAccStride;
-#else
-constexpr int X_ACC_END = X_CHO_END;
-#endif
 #if TRL_KIN_SMEM
-constexpr int X_PFX = (X_ACC_END + 1) & ~1;                 // three buffers of 32 double2: prefix rounds alternate 0 / 1, buffer 2 = (cos, sin) exchange
+constexpr int X_PFX = (X_CHO_END + 1) & ~1;                 // three buffers of 32 double2: prefix rounds alternate 0 / 1, buffer 2 = (cos, sin) exchange
 constexpr int X_PFX_END = X_PFX + 3 * 2 * kWarp;
 #else
-constexpr int X_PFX_END = X_ACC_END;
+constexpr int X_PFX_END = X_CHO_END;
 #endif
 #if TRL_OUTWARD_SMEM
 constexpr int X_BASE = (X_PFX_END + 1) & ~1;                // the 9 floating-base values of lane 0
@@ -136,13 +127,7 @@ constexpr int X_OUT_END = X_BASE + 10;
 #else
 constexpr int X_OUT_END = X_PFX_END;
 #endif
-#if TRL_CONTACT_SMEM
-constexpr int X_KIN = (X_OUT_END + 1) & ~1;                 // per-link (cw, sw) | (rx, ry) | (w, vx) as double2 [32] each, vy [32]
-constexpr int X_KIN_END = X_KIN + 7 * kWarp;
-#else
-constexpr int X_KIN_END = X_OUT_END;
-#endif
-constexpr int X_END = (X_KIN_END + 1) & ~1;
+constexpr int X_END = (X_OUT_END + 1) & ~1;
 // Measurement build (-DTRL_PHASE_CLOCKS=1, TRL_VARIANT=phase_clocks): lane 0 of every warp adds the clock64() delta of each
 // phase of the launch to g_phase_clocks[phase]; slot kNumPhases counts the physics halves (env-steps).  Read out by
 // trl_debug_step_phases (trl_probe.cu), printed by tools/step_phase_probe.py.  The product build compiles none of it.
@@ -1030,7 +1015,7 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
 // One sub-step of articulated-body forward dynamics with linearly-implicit contact / joint-limit terms.
 // Updates e (q, qd, root translation) in place and returns the contact bitmask (same value in every lane).
 __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g, const double* s_clx, const double* s_cly,
-                               const int* s_cbody, int lane, double dt, double clear_y, double* xs TRL_REUSE_KIN_DECL) {
+                               int lane, double dt, double clear_y, double* xs TRL_REUSE_KIN_DECL) {
     const double lk_mass = lc.mass;      // read once (shared-memory table; a read cannot move across the shuffles below)
     // per-body box tables (link frame): centre offset, axis rotation, half sizes -- staged by the kernel next to the corner tables
     const double *s_bax = s_clx + 4 * kMaxJoints, *s_bay = s_bax + kMaxJoints, *s_bc = s_bay + kMaxJoints, *s_bs = s_bc + kMaxJoints,
@@ -1059,25 +1044,15 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
     const double cvx = e.qd * (k.w * k.rx + k.vy), cvy = e.qd * (k.w * k.ry - k.vx);   // c_j = v_j x (S_j qd_j)
     TRL_CLK_END(PH_KIN, clk);
 
-    // ---- contacts: one box corner per lane per round against the height field
-    int contact = 0;
-    const int nc = m.n_corners;
-#if TRL_CONTACT_SMEM
-    // per-link kinematics staged once per sub-step; a corner lane reads the entries of the body it belongs to
-    double2* kin0 = trl_as2<double2>(xs + X_KIN);                  // (cw, sw)
-    double2* kin1 = trl_as2<double2>(xs + X_KIN + 2 * kWarp);      // (rx, ry)
-    double2* kin2 = trl_as2<double2>(xs + X_KIN + 4 * kWarp);      // (w, vx)
-    double* kin3 = xs + X_KIN + 6 * kWarp;                                   // vy
-    kin0[lane] = make_double2(k.cw, k.sw); kin1[lane] = make_double2(k.rx, k.ry);
-    kin2[lane] = make_double2(k.w, k.vx); kin3[lane] = k.vy;
-    __syncwarp();
-#endif
-    // one compliant contact at the point (rpx, rpy) rel. O of a body moving with (bw, bvx, bvy): penetration `pen` along the unit
-    // direction (nx, ny) the force pushes the body in; implicit in the point velocity (adds dt X^T D X to the body's articulated
-    // inertia and X^T w to its bias force, D = cnn n n^T + ctt t t^T)
-    auto contact_force = [&](double rpx, double rpy, double pen, double nx, double ny, double bw, double bvx, double bvy, double* add) {
+    // ---- contacts: the lane of each collidable body tests its own box against the height field, with the body's kinematics in its
+    // registers, and adds the forces straight into its articulated inertia: its 4 corners in corner order, then its vertex slots
+    // one compliant contact at the point (rpx, rpy) rel. O of the body: penetration `pen` along the unit direction (nx, ny) the force
+    // pushes the body in; implicit in the point velocity (adds dt X^T D X to the articulated inertia and X^T w to the bias force,
+    // D = cnn n n^T + ctt t t^T).  The sums are __dadd_rn so that no add is merged with the multiply that produced a term or the
+    // value it adds to: each contribution is rounded on its own, then added.
+    auto contact_force = [&](double rpx, double rpy, double pen, double nx, double ny) {
         const double tx = ny, ty = -nx;
-        const double pvx = bvx - bw * rpy, pvy = bvy + bw * rpx;
+        const double pvx = k.vx - k.w * rpy, pvy = k.vy + k.w * rpx;
         const double vn = pvx * nx + pvy * ny, vt = pvx * tx + pvy * ty;
         const double fn0 = pp.kn * pen - pp.dn * vn;
         if (fn0 > 0.0) {
@@ -1089,139 +1064,78 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
                          dyy = dt * (cnn * ny * ny + ctt * ty * ty);
             const double kx = -rpy, ky = rpx;
             const double dkx = dxx * kx + dxy * ky, dky = dxy * kx + dyy * ky;
-            add[0] = kx * dkx + ky * dky; add[1] = dkx; add[2] = dky; add[3] = dxx; add[4] = dxy; add[5] = dyy;
-            add[6] = -(rpx * fwy - rpy * fwx); add[7] = -fwx; add[8] = -fwy;
+            if (dxx != 0.0 || dyy != 0.0) {
+                // kx * dkx + ky * dky, spelled as the difference it is (kx = -rpy): written as a sum, the compiler fuses it into an FMA
+                // of its own choosing, which rounds differently
+                ia[0] = __dadd_rn(ia[0], ky * dky - dkx * rpy); ia[1] = __dadd_rn(ia[1], dkx); ia[2] = __dadd_rn(ia[2], dky);
+                ia[3] = __dadd_rn(ia[3], dxx); ia[4] = __dadd_rn(ia[4], dxy); ia[5] = __dadd_rn(ia[5], dyy);
+                ia[6] = __dadd_rn(ia[6], -(rpx * fwy - rpy * fwx)); ia[7] = __dadd_rn(ia[7], -fwx); ia[8] = __dadd_rn(ia[8], -fwy);
+            }
         }
     };
-    // rounds 0 .. nc/32: box corners against the height field.  rounds after that (pp.vertex_contacts): the terrain vertices inside a
-    // box -- lane (body, slot) looks at the slot-th vertex under the body's x extent (a box spans at most 4 vertices); where the surface
-    // is convex and the vertex lies inside, it is pushed out through the nearest face (sim/GroundVar2D.cpp:440-448 hands Bullet a
-    // height field: an edge of the terrain can enter a box between two of its corners)
-    const int nrounds = (nc + kWarp - 1) / kWarp;
-    for (int round = 0; round < (pp.vertex_contacts ? 2 * nrounds : nrounds); ++round) {
-        const bool vtx = round >= nrounds;
-        const int base = (vtx ? round - nrounds : round) * kWarp;
-        const int ci = base + lane;
-        const bool valid = ci < nc;
-        const int b = valid ? s_cbody[ci] : 0;
-        if (vtx) {
-            const double bcw = shf(k.cw, b), bsw = shf(k.sw, b), brx = shf(k.rx, b), bry = shf(k.ry, b);
-            const double bax = s_bax[b], bay = s_bay[b], bc = s_bc[b], bs = s_bs[b], hxb = s_hx[b], hyb = s_hy[b];
-            const double C = bcw * bc - bsw * bs, S = bsw * bc + bcw * bs;                      // box axes in the world
-            const double cxr = brx + bcw * bax - bsw * bay, cyr = bry + bsw * bax + bcw * bay;   // box centre rel. O
-            const bool cand = valid && (e.oy + cyr - (fabs(S) * hxb + fabs(C) * hyb) <= clear_y);
-            if (!__any_sync(kFull, cand)) continue;
-            const double bw = shf(k.w, b), bvx = shf(k.vx, b), bvy = shf(k.vy, b);
-            double add[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-            bool touching = false;
-            if (cand) {
-                const double extx = fabs(C) * hxb + fabs(S) * hyb, cxw = e.ox + cxr;
+    const int cb = lc.act ? LT(corner_base, lane) : -1;   // the body's 4 corners are cb .. cb + 3 of the corner tables
+    bool touching = false;
+    {
+        // box corners.  Broad phase: a corner above clear_y (terrain maximum under the character + margin) cannot be within the
+        // contact tolerance; a body with no candidate corner skips the height samples, a warp with none skips the pass.  The corner
+        // loop is unrolled by two, so two height samples are in flight at a time (unrolled by four, the kernel spills more)
+        const int c0 = cb >= 0 ? cb : 0;
+        unsigned cand = 0;
+#pragma unroll
+        for (int cn = 0; cn < 4; ++cn) {
+            const double ly = s_cly[c0 + cn], rpy = k.ry + k.sw * s_clx[c0 + cn] + k.cw * ly;
+            if (cb >= 0 && (e.oy + rpy <= clear_y)) cand |= 1u << cn;
+        }
+        if (__any_sync(kFull, cand != 0) && cand) {
+#pragma unroll 2
+            for (int cn = 0; cn < 4; ++cn) {
+                if (!((cand >> cn) & 1u)) continue;
+                const double lx = s_clx[c0 + cn], ly = s_cly[c0 + cn];
+                const double rpx = k.rx + k.cw * lx - k.sw * ly, rpy = k.ry + k.sw * lx + k.cw * ly;   // corner rel. O
+                double slope;
+                const double hgt = g.sample_fast(e.ox + rpx, &slope);
+                const double inv = rsqrt(1.0 + slope * slope);
+                const double pen = (hgt - (e.oy + rpy)) * inv;
+                if (pen > -pp.contact_tol) {
+                    touching = true;
+                    if (pen > 0.0) contact_force(rpx, rpy, pen, -slope * inv, inv);
+                }
+            }
+        }
+    }
+    if (pp.vertex_contacts) {
+        // the terrain vertices inside the box (opt-in), after the corners: slot s is the s-th vertex under the body's x extent (a
+        // box spans at most 4 vertices); where the surface is convex and the vertex lies inside, it is pushed out through the nearest
+        // face (sim/GroundVar2D.cpp:440-448 hands Bullet a height field: an edge of the terrain can enter a box between two of its
+        // corners)
+        const int j = cb >= 0 ? lane : 0;
+        const double bax = s_bax[j], bay = s_bay[j], bc = s_bc[j], bs = s_bs[j], hxb = s_hx[j], hyb = s_hy[j];
+        const double C = k.cw * bc - k.sw * bs, S = k.sw * bc + k.cw * bs;                        // box axes in the world
+        const double cxr = k.rx + k.cw * bax - k.sw * bay, cyr = k.ry + k.sw * bax + k.cw * bay;   // box centre rel. O
+        const bool cand = cb >= 0 && (e.oy + cyr - (fabs(S) * hxb + fabs(C) * hyb) <= clear_y);
+        if (__any_sync(kFull, cand) && cand) {
+            const double extx = fabs(C) * hxb + fabs(S) * hyb, cxw = e.ox + cxr;
+#pragma unroll 1
+            for (int slot = 0; slot < 4; ++slot) {
                 double xv, hv, hp, hn;
-                if (g.vertex_slot(cxw - extx - pp.contact_tol, cxw + extx + pp.contact_tol, ci & 3, &xv, &hv, &hp, &hn) && hv - 0.5 * (hp + hn) > 1e-9) {
-                    const double rx = xv - cxw, ry = hv - (e.oy + cyr);
-                    const double lx = C * rx + S * ry, ly = -S * rx + C * ry;
-                    const double dx = hxb - fabs(lx), dy = hyb - fabs(ly);
-                    if (dx > -pp.contact_tol && dy > -pp.contact_tol) {
-                        touching = true;
-                        if (dx > 0.0 && dy > 0.0) {
-                            double nlx = 0.0, nly = 0.0, pen;
-                            if (dx < dy) { nlx = lx > 0.0 ? -1.0 : 1.0; pen = dx; } else { nly = ly > 0.0 ? -1.0 : 1.0; pen = dy; }
-                            contact_force(xv - e.ox, hv - e.oy, pen, C * nlx - S * nly, S * nlx + C * nly, bw, bvx, bvy, add);
-                        }
+                if (!g.vertex_slot(cxw - extx - pp.contact_tol, cxw + extx + pp.contact_tol, slot, &xv, &hv, &hp, &hn) ||
+                    !(hv - 0.5 * (hp + hn) > 1e-9))
+                    continue;
+                const double rx = xv - cxw, ry = hv - (e.oy + cyr);
+                const double lx = C * rx + S * ry, ly = -S * rx + C * ry;
+                const double dx = hxb - fabs(lx), dy = hyb - fabs(ly);
+                if (dx > -pp.contact_tol && dy > -pp.contact_tol) {
+                    touching = true;
+                    if (dx > 0.0 && dy > 0.0) {
+                        double nlx = 0.0, nly = 0.0, pen;
+                        if (dx < dy) { nlx = lx > 0.0 ? -1.0 : 1.0; pen = dx; } else { nly = ly > 0.0 ? -1.0 : 1.0; pen = dy; }
+                        contact_force(xv - e.ox, hv - e.oy, pen, C * nlx - S * nly, S * nlx + C * nly);
                     }
                 }
             }
-            const unsigned tmask = __ballot_sync(kFull, touching);
-            unsigned fmask = __ballot_sync(kFull, add[3] != 0.0 || add[5] != 0.0);
-            const int cb = lc.act ? LT(corner_base, lane) : -1;
-            const bool mine = cb >= base && cb < base + kWarp;
-            while (fmask) {
-                const int src = __ffs(fmask) - 1;
-                fmask &= fmask - 1;
-                const bool to_me = mine && (src >= cb - base) && (src < cb - base + 4);
-#pragma unroll
-                for (int v = 0; v < 9; ++v) {
-                    double t = shf(add[v], src);
-                    if (to_me) ia[v] += t;
-                }
-            }
-            if (mine && ((tmask >> (cb - base)) & 0xfu)) contact |= 1 << lane;
-            continue;
         }
-        const double lx = valid ? s_clx[ci] : 0.0, ly = valid ? s_cly[ci] : 0.0;
-#if TRL_CONTACT_SMEM
-        const double2 k0_ = kin0[b], k1_ = kin1[b];
-        const double bcw = k0_.x, bsw = k0_.y, brx = k1_.x, bry = k1_.y;
-#else
-        const double bcw = shf(k.cw, b), bsw = shf(k.sw, b), brx = shf(k.rx, b), bry = shf(k.ry, b);
-#endif
-        const double rpx = brx + bcw * lx - bsw * ly, rpy = bry + bsw * lx + bcw * ly;   // corner rel. O
-        // broad phase: a corner above clear_y (terrain maximum under the character + margin) cannot be within the
-        // contact tolerance; a round with no candidate corner is skipped by the whole warp
-        const bool cand = valid && (e.oy + rpy <= clear_y);
-        if (!__any_sync(kFull, cand)) continue;
-#if TRL_CONTACT_SMEM
-        const double2 k2_ = kin2[b];
-        const double bw = k2_.x, bvx = k2_.y, bvy = kin3[b];
-#else
-        const double bw = shf(k.w, b), bvx = shf(k.vx, b), bvy = shf(k.vy, b);
-#endif
-        double add[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-        bool touching = false;
-        if (cand) {
-            double slope;
-            const double hgt = g.sample_fast(e.ox + rpx, &slope);
-            const double inv = rsqrt(1.0 + slope * slope);
-            const double pen = (hgt - (e.oy + rpy)) * inv;
-            if (pen > -pp.contact_tol) {
-                touching = true;
-                if (pen > 0.0) contact_force(rpx, rpy, pen, -slope * inv, inv, bw, bvx, bvy, add);
-            }
-        }
-        // hand the (few) force-producing corners to the lanes that own their bodies, in corner order (deterministic)
-        const unsigned tmask = __ballot_sync(kFull, touching);
-        unsigned fmask = __ballot_sync(kFull, add[3] != 0.0 || add[5] != 0.0);
-        const int cb = lc.act ? LT(corner_base, lane) : -1;
-        const bool mine = cb >= base && cb < base + kWarp;
-#if TRL_CONTACT_SMEM
-        if (fmask) {
-            // force-producing corner lanes publish their 9 values; the lane that owns the body adds its (up to 4) corners in
-            // corner order -- the order the shuffle loop below visits them in
-            double* slot = xs + X_ACC + lane * kAccStride;
-            if ((fmask >> lane) & 1u) {
-                double2* s2 = trl_as2<double2>(slot);
-                s2[0] = make_double2(add[0], add[1]); s2[1] = make_double2(add[2], add[3]); s2[2] = make_double2(add[4], add[5]);
-                s2[3] = make_double2(add[6], add[7]); slot[8] = add[8];
-            }
-            __syncwarp();
-            const unsigned my = mine ? ((fmask >> (cb - base)) & 0xfu) : 0u;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                if ((my >> q) & 1u) {
-                    const double* from = xs + X_ACC + (cb - base + q) * kAccStride;
-                    const double2* f2 = trl_as2<const double2>(from);
-                    const double2 t0 = f2[0], t1 = f2[1], t2 = f2[2], t3 = f2[3];
-                    ia[0] += t0.x; ia[1] += t0.y; ia[2] += t1.x; ia[3] += t1.y; ia[4] += t2.x; ia[5] += t2.y;
-                    ia[6] += t3.x; ia[7] += t3.y; ia[8] += from[8];
-                }
-            }
-            __syncwarp();
-        }
-#else
-        while (fmask) {
-            const int src = __ffs(fmask) - 1;
-            fmask &= fmask - 1;
-            const bool to_me = mine && (src >= cb - base) && (src < cb - base + 4);
-#pragma unroll
-            for (int v = 0; v < 9; ++v) {
-                double t = shf(add[v], src);
-                if (to_me) ia[v] += t;
-            }
-        }
-#endif
-        if (mine && ((tmask >> (cb - base)) & 0xfu)) contact |= 1 << lane;
     }
-    contact = (int)__ballot_sync(kFull, contact != 0);   // lane index == link index
+    const int contact = (int)__ballot_sync(kFull, touching);   // lane index == link index
     TRL_CLK_END(PH_CONTACT, clk);
 
     // ---- articulated-body forward dynamics over the chain schedule
@@ -1366,12 +1280,11 @@ __device__ __forceinline__ void catchup_leave(const Buffers& B, int prev) {
 __global__ void __launch_bounds__(kBlockThreads, TRL_STEP_MIN_BLOCKS)
 trl_step_kernel(Buffers B, double h, int flags, int lists) {
     __shared__ double s_clx[4 * kMaxJoints + 6 * kMaxJoints], s_cly[4 * kMaxJoints];     // s_clx also carries the six per-body box tables
-    __shared__ int s_cbody[4 * kMaxJoints];
     __shared__ __align__(16) double s_x[kWarpsPerBlock * X_END];
     TRL_CLK_BEGIN(clk);
     const ModelConst& m = c_model;
     for (int t = threadIdx.x; t < m.n_corners; t += kBlockThreads) {
-        s_clx[t] = LT(corner_lx, t); s_cly[t] = LT(corner_ly, t); s_cbody[t] = LT(corner_body, t);
+        s_clx[t] = LT(corner_lx, t); s_cly[t] = LT(corner_ly, t);
     }
     for (int t = threadIdx.x; t < m.nj; t += kBlockThreads) {
         double* tb = s_clx + 4 * kMaxJoints;
@@ -1539,9 +1452,9 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         const double clear_y = g.window_max(e.ox - m.reach - 0.25, e.ox + m.reach + 0.25, lane) + kClearMargin;
 #if TRL_REUSE_KIN
         for (int s = 0; s < ns; ++s)
-            contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y, xs, (s == 0 && have_k) ? &k_ctrl : nullptr);
+            contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs, (s == 0 && have_k) ? &k_ctrl : nullptr);
 #else
-        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, s_cbody, lane, dt, clear_y, xs);
+        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs);
 #endif
         TRL_CLK_RESET(clk);
         // UpdateGround (scenarios/ScenarioSimChar.cpp:564-572): regenerate a segment when the view window crosses it

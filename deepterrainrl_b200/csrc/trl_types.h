@@ -107,7 +107,6 @@ struct ModelConst {
     int chain_merge[kMaxJoints];           // 5 bits per child chain summed into the bottom link, in summation order (31 = none)
     int chain_up[kMaxJoints];              // parent link of the chain's top link (-1 for the root's chain)
     int n_corners;                         // 4 * number of collidable bodies
-    int corner_body[4 * kMaxJoints];
     double corner_lx[4 * kMaxJoints], corner_ly[4 * kMaxJoints];   // corner position in the link (joint) frame
     int corner_base[kMaxJoints];           // first corner index of a body (-1 if not collidable)
     double reach;                          // upper bound of |box corner - root joint| over all poses

@@ -25,8 +25,6 @@ NVCC_FLAGS = ARCH_FLAGS + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPI
 VARIANTS = {
     "kin_smem": ["-DTRL_KIN_SMEM=1"],
     "outward_smem": ["-DTRL_OUTWARD_SMEM=1"],    # since the chain passes: only the floating-base broadcast (parent -> child accelerations always use the link block)
-    "contact_smem": ["-DTRL_CONTACT_SMEM=1"],
-    "xchg_no_contact": ["-DTRL_KIN_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],
     "smem_xchg": ["-DTRL_SMEM_XCHG=1"],
     "smem_xchg_3cta": ["-DTRL_SMEM_XCHG=1", "-DTRL_STEP_MIN_BLOCKS=3"],
     "noinline_cold": ["-DTRL_NOINLINE_COLD=1"],
@@ -38,7 +36,6 @@ VARIANTS = {
     "cta2": ["-DTRL_WARPS_PER_BLOCK=2", "-DTRL_STEP_MIN_BLOCKS=8"],
     "cta8": ["-DTRL_WARPS_PER_BLOCK=8", "-DTRL_STEP_MIN_BLOCKS=2"],
     "table_const": ["-DTRL_TABLE_MIRROR=0"],     # lane-indexed model tables from constant memory (divergent LDC, the round-1 reads); the default reads a global-memory mirror
-    "contact_outward_smem": ["-DTRL_CONTACT_SMEM=1", "-DTRL_OUTWARD_SMEM=1"],   # outward part: the floating-base broadcast only (see outward_smem)
     "link_regs": ["-DTRL_LINK_SMEM=0"],          # the round-1 layout: per-lane link constants in registers (the default keeps them in shared memory)          # per-lane link constants in shared memory instead of ~28 registers (180 B instead of 216 B spilled)
     "reuse_kin": ["-DTRL_REUSE_KIN=1"],
     "smem_xchg_reuse_kin": ["-DTRL_SMEM_XCHG=1", "-DTRL_REUSE_KIN=1"],
