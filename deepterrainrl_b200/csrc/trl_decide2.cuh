@@ -212,6 +212,82 @@ trl_decide_conv_kernel(Buffers B, NetWeights W, double* __restrict__ act2, int l
     }
 }
 
+// slot build: the same stage with the weights and input offset / scale of the env's policy slot
+__global__ void __cluster_dims__(kClusterSize, 1, 1) __launch_bounds__(kDecideThreads, 2)
+trl_decide_conv_slots_kernel(Buffers B, PolicySlots P, double* __restrict__ act2, int list) {
+    TRL_DYN_SHARED(double, sh);
+    cg::cluster_group cluster = cg::this_cluster();
+    const ModelConst& m = c_model;
+    if (!m.has_net) return;
+    const int cid = blockIdx.x / kClusterSize, ncl = gridDim.x / kClusterSize;
+    const int count = B.pending_count[list];
+    for (int idx = cid; idx < count; idx += ncl) {
+        const int env = B.pending_list[list * B.n + idx];
+        conv_stage_cluster(cluster, P.W[P.env_slot[env]], B.poli_state + (size_t)env * B.S, sh, m.n_char, act2 + (size_t)idx * kTipIn);
+    }
+}
+
+// Slot build, ahead of the conv stage: regroups pending list `list` by policy slot (a counting sort in one CTA; the order within a
+// slot is whatever the atomics give -- every row of the pass is independent of the others, and so is the catch-up launch that
+// reads the list afterwards) and writes the FC stage's chunk table: each 32-row chunk belongs to one slot, a slot's last chunk
+// may be ragged.
+__global__ void __launch_bounds__(1024) trl_slot_sort_kernel(Buffers B, PolicySlots P, int* __restrict__ tmp, int* __restrict__ tab, int list) {
+    __shared__ int cnt[kMaxPolicySlots], next[kMaxPolicySlots];
+    const int count = B.pending_count[list];
+    int* L = B.pending_list + (size_t)list * B.n;
+    if (threadIdx.x < kMaxPolicySlots) cnt[threadIdx.x] = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < count; i += blockDim.x) {
+        const int env = L[i];
+        tmp[i] = env;
+        atomicAdd(&cnt[P.env_slot[env]], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int row = 0, nc = 0;
+        for (int p = 0; p < kMaxPolicySlots; ++p) {
+            next[p] = row;
+            for (int r = 0; r < cnt[p]; r += kFcRows, ++nc) {
+                tab[1 + 3 * nc] = p; tab[2 + 3 * nc] = row + r; tab[3 + 3 * nc] = min(kFcRows, cnt[p] - r);
+            }
+            row += cnt[p];
+        }
+        tab[0] = nc;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < count; i += blockDim.x) {
+        const int env = tmp[i];
+        L[atomicAdd(&next[P.env_slot[env]], 1)] = env;
+    }
+}
+
+// cycles / episodes / env-steps / episode-weighted distance of each policy slot's envs into out[kMaxPolicySlots][4], one slot after
+// the other with trl_stats_kernel's reduction (env_slot null: every env is on slot 0)
+__global__ void __launch_bounds__(1024) trl_slot_stats_kernel(Buffers B, const int* __restrict__ env_slot, double* __restrict__ out) {
+    __shared__ double red[4][32];
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
+    for (int p = 0; p < kMaxPolicySlots; ++p) {
+        double c = 0, e = 0, st = 0, ds = 0;
+        for (int env = threadIdx.x; env < B.n; env += blockDim.x) {
+            if ((env_slot ? env_slot[env] : 0) != p) continue;
+            const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
+            c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
+            e += ec;
+            st += (double)(((uint64_t)(uint32_t)B.i[(size_t)I_STEPS_HI * B.n + env] << 32) | (uint32_t)B.i[(size_t)I_STEPS_LO * B.n + env]);
+            ds += B.d[(size_t)D_AVG_DIST * B.n + env] * ec;
+        }
+        c = warp_sum_all(c); e = warp_sum_all(e); st = warp_sum_all(st); ds = warp_sum_all(ds);
+        if (l == 0) { red[0][w] = c; red[1][w] = e; red[2][w] = st; red[3][w] = ds; }
+        __syncthreads();
+        if (w == 0)
+            for (int k = 0; k < 4; ++k) {
+                const double v = warp_sum_all(l < nw ? red[k][l] : 0.0);
+                if (l == 0) out[4 * p + k] = v;
+            }
+        __syncthreads();
+    }
+}
+
 // the conv stage over the rows of a trainer minibatch (one cluster per row)
 __global__ void __cluster_dims__(kClusterSize, 1, 1) __launch_bounds__(kDecideThreads, 2)
 trl_fwd_conv_train_kernel(NetWeights W, FwdTrain f, double* __restrict__ act2) {
@@ -283,9 +359,12 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
     store_rng(L, rng);
 }
 
-template <bool kTrain>
-__device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, const ExpSettings* __restrict__ ex_dev, const FcMaps& maps, const FwdTrain& ft,
-                                         int* done_count, int list, int rearm) {
+// kSlots: the slot build (trl_decide_fc_slots_kernel).  The chunks come from the table trl_slot_sort_kernel wrote, each with its slot's
+// weights (W0 = the slot table), terr_ip0 descriptor (smaps) and output offset / scale; the ip0 weight slice is restaged when a
+// cluster moves on to a chunk of another slot.  Without it, the single-policy kernel: chunk k = rows 32 k .., W0 = the one net.
+template <bool kTrain, bool kSlots = false>
+__device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0, const ExpSettings* __restrict__ ex_dev, const FcMaps& maps, const FwdTrain& ft,
+                                         int* done_count, int list, int rearm, const FcSlotMaps* smaps = nullptr, const int* __restrict__ tab = nullptr) {
     TRL_DYN_SHARED(unsigned char, fc_smem_raw);
     // the swizzled TMA tiles need 1024-byte alignment; the dynamic window starts at the same offset in every CTA of the cluster, so
     // the rounded address is a valid DSMEM offset as well
@@ -314,7 +393,7 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, 
     double* Y = (double*)(fc_smem + kFcOffY);
     unsigned long long* bar_full = (unsigned long long*)(fc_smem + kFcOffBar);
     unsigned long long* bar_empty = bar_full + kFcStages;
-    const int nchunks = (count + kFcRows - 1) / kFcRows;
+    const int nchunks = kSlots ? tab[0] : (count + kFcRows - 1) / kFcRows;
     int prof_n = 0;
     auto stamp = [&]() {
 #ifndef TRL_SIMT_EMU
@@ -329,10 +408,11 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, 
 
     if (has_net && cid < nchunks) {
         // ip0 weight slice of this CTA (32 output columns x ncat, zero-padded to kCatStride): resident for the whole launch
-        for (int i = tid; i < 32 * kCatStride; i += kFcThreads) {
-            const int n = i / kCatStride, k = i - n * kCatStride;
-            WIP[i] = k < ncat ? W.ip0_w[(size_t)(rank * 32 + n) * ncat + k] : 0.0;
-        }
+        if (!kSlots)
+            for (int i = tid; i < 32 * kCatStride; i += kFcThreads) {
+                const int n = i / kCatStride, k = i - n * kCatStride;
+                WIP[i] = k < ncat ? W0.ip0_w[(size_t)(rank * 32 + n) * ncat + k] : 0.0;
+            }
 #ifndef TRL_SIMT_EMU
         if (tid == 0) {
             for (int s = 0; s < kFcStages; ++s) { mbar_init(&bar_full[s], 1); mbar_init(&bar_empty[s], kFcThreads / 32); }
@@ -346,10 +426,22 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, 
     // k tiles of terr_ip0 this CTA multiplies
     const int kt0 = (kNumKTiles * rank) / kFcCluster, kt1 = (kNumKTiles * (rank + 1)) / kFcCluster;
     unsigned pipe_iter = 0;      // tiles issued / consumed so far over all chunks (stage = iter % kFcStages, parity from iter / kFcStages)
+    int staged = -1;             // slot build: the slot whose ip0 slice WIP holds
 
     for (int chunk = cid; chunk < nchunks; chunk += ncl) {
-        const int row0 = chunk * kFcRows;
-        const int rows = min(kFcRows, count - row0);
+        const int slot = kSlots ? tab[1 + 3 * chunk] : 0;
+        const int row0 = kSlots ? tab[2 + 3 * chunk] : chunk * kFcRows;
+        const int rows = kSlots ? tab[3 + 3 * chunk] : min(kFcRows, count - row0);
+        const NetWeights& W = kSlots ? (&W0)[slot] : W0;
+        if (kSlots && has_net && slot != staged) {
+            // WIP was last read by the previous chunk's ip0, before its closing cluster.sync; the cluster.sync behind terr_ip0 below
+            // orders these writes before this chunk's reads
+            for (int i = tid; i < 32 * kCatStride; i += kFcThreads) {
+                const int n = i / kCatStride, k = i - n * kCatStride;
+                WIP[i] = k < ncat ? W.ip0_w[(size_t)(rank * 32 + n) * ncat + k] : 0.0;
+            }
+            staged = slot;
+        }
         if (has_net) {
             // ---------------- terr_ip0: P[32][64] = A[32][k slice] * Wt[k slice][64]; warp w owns C tiles (m tile w / 4, n tiles 2 (w % 4) + {0, 1})
             const int mt = warp >> 2, nt0 = (warp & 3) * 2;
@@ -368,7 +460,7 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, 
                 mbar_expect_tx(&bar_full[s], nt * kTileBytes);
                 for (int q = 0; q < nt; ++q) {
                     const int kt = kt0 + j * kTilesPerStage + q;
-                    tma_load_2d(st + q * kTileBytes, &maps.w, &bar_full[s], kt * kKT, 0);
+                    tma_load_2d(st + q * kTileBytes, kSlots ? &smaps->w[slot] : &maps.w, &bar_full[s], kt * kKT, 0);
                     tma_load_2d(st + q * kTileBytes + kWTileBytes, &maps.a, &bar_full[s], kt * kKT, row0);
                 }
             };
@@ -392,7 +484,7 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W, 
                     const int kt = kt0 + j * kTilesPerStage + q;
                     for (int i = tid; i < kTip0Out * kKT; i += kFcThreads) {
                         const int n = i / kKT, k = i - n * kKT;
-                        Wq[swz(n, k)] = maps.w_ptr[(size_t)n * kTipIn + kt * kKT + k];
+                        Wq[swz(n, k)] = (kSlots ? smaps->w_ptr[slot] : maps.w_ptr)[(size_t)n * kTipIn + kt * kKT + k];
                     }
                     for (int i = tid; i < kFcRows * kKT; i += kFcThreads) {
                         const int r = i / kKT, k = i - r * kKT;
@@ -560,6 +652,13 @@ trl_decide_fc_kernel(Buffers B, NetWeights W, const ExpSettings* __restrict__ ex
     const FwdTrain none{};
     fc_stage<false>(B, W, ex_dev, maps, none, done_count, list, rearm);
 }
+// slot build: chunks from the table of trl_slot_sort_kernel, weights of each chunk's slot
+__global__ void __cluster_dims__(kFcCluster, 1, 1) __launch_bounds__(kFcThreads, 1)
+trl_decide_fc_slots_kernel(Buffers B, PolicySlots P, const ExpSettings* __restrict__ ex_dev, const TRL_GRID_CONSTANT FcMaps maps,
+                           const TRL_GRID_CONSTANT FcSlotMaps smaps, const int* __restrict__ tab, int* done_count, int list, int rearm) {
+    const FwdTrain none{};
+    fc_stage<false, true>(B, *P.W, ex_dev, maps, none, done_count, list, rearm, &smaps, tab);
+}
 // the FC stage over a trainer minibatch: activations and raw outputs to global memory, no decisions
 __global__ void __cluster_dims__(kFcCluster, 1, 1) __launch_bounds__(kFcThreads, 1)
 trl_fwd_fc_train_kernel(NetWeights W, const TRL_GRID_CONSTANT FcMaps maps, FwdTrain f) {
@@ -573,6 +672,8 @@ cudaError_t configure_decide2_kernels() {
     cudaError_t e = cudaFuncSetAttribute(trl_decide_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmemDoubles * 8);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(trl_fwd_conv_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmemDoubles * 8);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(trl_fwd_fc_train_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decide_fc_smem_bytes());
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(trl_decide_conv_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmemDoubles * 8);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(trl_decide_fc_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decide_fc_smem_bytes());
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(trl_decide_fc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)decide_fc_smem_bytes());
 }
@@ -583,6 +684,22 @@ void launch_decide2(const Buffers& B, const NetWeights& W, const ExpSettings* ex
     if (part & 2)
         TRL_LAUNCH_CLUSTER(kFcCluster, trl_decide_fc_kernel, fc_clusters * kFcCluster, kFcThreads, decide_fc_smem_bytes(), st, B, W, ex, maps, done_count,
                            list, rearm);
+}
+
+// slot build of the same pass: regroup the list by slot (part 1, before the conv stage), conv stage, FC stage over the chunk table
+// tab (one per side stream, like act2)
+void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSettings* ex, const FcMaps& maps, const FcSlotMaps& smaps, double* act2,
+                          int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part) {
+    if (part & 1) {
+        TRL_LAUNCH(trl_slot_sort_kernel, 1, 1024, 0, st, B, P, tmp, tab, list);
+        TRL_LAUNCH_CLUSTER(kClusterSize, trl_decide_conv_slots_kernel, grid, kDecideThreads, (size_t)kConvSmemDoubles * 8, st, B, P, act2, list);
+    }
+    if (part & 2)
+        TRL_LAUNCH_CLUSTER(kFcCluster, trl_decide_fc_slots_kernel, fc_clusters * kFcCluster, kFcThreads, decide_fc_smem_bytes(), st, B, P, ex, maps, smaps,
+                           (const int*)tab, done_count, list, rearm);
+}
+void launch_slot_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st) {
+    TRL_LAUNCH(trl_slot_stats_kernel, 1, 1024, 0, st, B, env_slot, out);
 }
 
 // the forward pass of a trainer minibatch through the same two kernels (trl_train.cu: enqueue_forward); act2 = [rows][5984] scratch the

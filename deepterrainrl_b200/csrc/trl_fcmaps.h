@@ -20,6 +20,14 @@ struct FcMaps {
     unsigned long long* prof;    // measurement only (trl_debug_fc_phases): rank 0 / thread 0 of cluster 0 stamps %globaltimer at phase ends
 };
 
+// the terr_ip0 weight descriptor of every policy slot (slot build of the FC kernel; 8 x 128 B, a __grid_constant__ parameter)
+struct FcSlotMaps {
+#ifndef TRL_SIMT_EMU
+    CUtensorMap w[8];
+#endif
+    const double* w_ptr[8];
+};
+
 // the same two kernels as the forward pass of a TRAINER batch (trl_train.cu): rows = the minibatch, inputs already normalised, every
 // activation the backward pass needs written out, raw (normalised) outputs, no decisions.  All-null in the decision path.
 struct FwdTrain {

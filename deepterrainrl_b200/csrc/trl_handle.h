@@ -45,6 +45,17 @@ struct trl_handle {
     trl::FcMaps fc_maps[8];
     const double* fc_maps_w = nullptr;
     int fc_clusters = 2;
+    // policy slots (trl_load_policy, evaluation handles only): slot 0 is W / net_blobs above, slots 1.. own their blobs.  While any
+    // slot >= 1 is loaded (slots_active) every decision goes through the slot build of the decision kernels; before that nothing below
+    // is allocated and the single-policy kernels run
+    bool slots_active = false;
+    bool slot_dirty = false;                                 // a slot was (re)loaded: device table and descriptors to be rewritten
+    std::vector<double*> slot_blobs[trl::kMaxPolicySlots];   // [0] unused
+    trl::NetWeights slot_W[trl::kMaxPolicySlots] = {};       // [0] mirrors W when the device table was last written
+    std::vector<int> env_slot_host;
+    trl::PolicySlots P{};                                    // device views (env_slot, weight table, sort scratch, chunk tables)
+    trl::FcSlotMaps slot_maps{};
+    double* slot_stats = nullptr;                            // [kMaxPolicySlots][4]
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
     bool use_graph = true;
@@ -66,6 +77,12 @@ struct trl_handle {
     double* snap_host = nullptr;     // pinned mirror
     bool snap_pending = false;
 };
+
+// the weights the decisions of `env` use
+inline const trl::NetWeights& env_policy(const trl_handle* h, int env) {
+    const int p = h->slots_active ? h->env_slot_host[env] : 0;
+    return p == 0 ? h->W : h->slot_W[p];
+}
 
 // shared by the translation units behind the C ABI
 int trl_fail(const std::string& msg);                 // records the message for trl_last_error(), returns 1

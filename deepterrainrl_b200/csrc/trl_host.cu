@@ -33,6 +33,9 @@ size_t decide_fc_smem_bytes();
 cudaError_t configure_decide2_kernels();
 void launch_decide2(const Buffers& B, const NetWeights& W, const ExpSettings* ex, const FcMaps& maps, double* act2, int* done_count, int grid,
                     int fc_clusters, int list, int rearm, cudaStream_t st, int part);
+void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSettings* ex, const FcMaps& maps, const FcSlotMaps& smaps, double* act2,
+                          int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part);
+void launch_slot_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
@@ -70,10 +73,12 @@ static const char* kNetLayers[13] = {"terr_conv0", "terr_conv1", "terr_conv2", "
 // The kernels read the scene from __constant__ memory, of which there is one copy per process: a handle that is not the
 // current owner re-uploads its model (after draining the owner's work) before it launches anything.
 static int ensure_fc_maps(trl_handle* h);
+static int ensure_slot_tables(trl_handle* h);
 static int ensure_model_only(trl_handle* h);
 static int ensure_model(trl_handle* h) {
     if (ensure_model_only(h)) return 1;
-    return ensure_fc_maps(h);
+    if (ensure_fc_maps(h)) return 1;
+    return ensure_slot_tables(h);
 }
 static int ensure_model_only(trl_handle* h) {
     // one process drives one GPU (DESIGN.md §7): __constant__ scene memory and the streams belong to the device of the handle
@@ -332,26 +337,28 @@ static int fill_model(trl_handle* h, uint64_t rng_seed) {
     return 0;
 }
 
-static int upload_net(trl_handle* h, const double* const* blobs, const int64_t* counts, const double* const* vecs4, const int64_t* vcounts) {
+// into policy slot `slot` (0: the handle's own net, W); every slot has the topology of the first upload
+static int upload_net(trl_handle* h, const double* const* blobs, const int64_t* counts, const double* const* vecs4, const int64_t* vcounts,
+                      int slot = 0) {
     // blobs: 26 (w, b per layer), vecs4: in_off, in_scale, out_off, out_scale
-    if (h->net_blobs.empty()) {
-        h->net_blobs.assign(30, nullptr);
+    std::vector<double*>& dst = slot == 0 ? h->net_blobs : h->slot_blobs[slot];
+    if (h->net_counts.empty()) {
         h->net_counts.assign(30, 0);
-        for (int i = 0; i < 30; ++i) {
-            int64_t c = i < 26 ? counts[i] : vcounts[i - 26];
-            h->net_counts[i] = c;
-            CK(dalloc(h, &h->net_blobs[i], (size_t)c));
-        }
+        for (int i = 0; i < 30; ++i) h->net_counts[i] = i < 26 ? counts[i] : vcounts[i - 26];
+    }
+    if (dst.empty()) {
+        dst.assign(30, nullptr);
+        for (int i = 0; i < 30; ++i) CK(dalloc(h, &dst[i], (size_t)h->net_counts[i]));
     }
     for (int i = 0; i < 30; ++i) {
         int64_t c = i < 26 ? counts[i] : vcounts[i - 26];
         if (c != h->net_counts[i]) return fail("trl_set_weights: blob size mismatch");
         const double* src = i < 26 ? blobs[i] : vecs4[i - 26];
-        CK(cudaMemcpyAsync(h->net_blobs[i], src, (size_t)c * 8, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(dst[i], src, (size_t)c * 8, cudaMemcpyHostToDevice, h->stream));
     }
     CK(cudaStreamSynchronize(h->stream));
-    double** b = h->net_blobs.data();
-    h->W = net_weights(b, b[26], b[27], b[28], b[29]);
+    double** b = dst.data();
+    (slot == 0 ? h->W : h->slot_W[slot]) = net_weights(b, b[26], b[27], b[28], b[29]);
     return 0;
 }
 
@@ -432,16 +439,39 @@ static int ensure_fc_maps(trl_handle* h) {
     h->fc_maps_w = h->W.tip0_w;
     return 0;
 }
-// the decision launch(es) of one env-step
-static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, int part = 3, int slot = 0) {
-    if (h->decide_v2)
-        launch_decide2(h->B, h->W, h->d_ex, h->fc_maps[slot], h->act2[slot], h->done_count, h->decide_grid, h->fc_clusters, list, rearm, st, part);
+static void destroy_graphs(trl_handle* h);
+// slot build: the device table of the slots' weights and each slot's terr_ip0 descriptor, rewritten after a slot was loaded or slot 0's
+// weights moved.  Captured graphs bake the descriptors in and are dropped.  Called with the handle drained.
+static int ensure_slot_tables(trl_handle* h) {
+    if (!h->slots_active) return 0;
+    if (!h->slot_dirty && std::memcmp(&h->slot_W[0], &h->W, sizeof(NetWeights)) == 0) return 0;
+    h->slot_W[0] = h->W;
+    CK(cudaMemcpy((void*)h->P.W, h->slot_W, sizeof(h->slot_W), cudaMemcpyHostToDevice));
+    for (int p = 0; p < kMaxPolicySlots; ++p) {
+        const double* w = h->slot_W[p].tip0_w;
+        if (!w || h->slot_maps.w_ptr[p] == w) continue;
+#ifndef TRL_SIMT_EMU
+        if (encode_rows_map(&h->slot_maps.w[p], w, 64, 64)) return 1;
+#endif
+        h->slot_maps.w_ptr[p] = w;
+    }
+    destroy_graphs(h);
+    h->slot_dirty = false;
+    return 0;
+}
+// the decision launch(es) of one env-step; `side` = the side stream's index (its act2 scratch, descriptors and chunk table)
+static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, int part = 3, int side = 0) {
+    if (h->decide_v2 && h->slots_active)
+        launch_decide2_slots(h->B, h->P, h->d_ex, h->fc_maps[side], h->slot_maps, h->act2[side], h->P.sort_tmp + (size_t)side * h->n,
+                             h->P.chunks + (size_t)side * (1 + 3 * h->P.chunk_cap), h->done_count, h->decide_grid, h->fc_clusters, list, rearm, st,
+                             part);
+    else if (h->decide_v2)
+        launch_decide2(h->B, h->W, h->d_ex, h->fc_maps[side], h->act2[side], h->done_count, h->decide_grid, h->fc_clusters, list, rearm, st, part);
     else if (part & 1)
         launch_decide(h->B, h->W, h->d_ex, h->done_count, h->decide_grid, list, rearm, st);
 }
-static int num_decide_launches(const trl_handle* h) { return h->decide_v2 ? 2 : 1; }
+static int num_decide_launches(const trl_handle* h) { return h->decide_v2 ? (h->slots_active ? 3 : 2) : 1; }
 
-static void destroy_graphs(trl_handle* h);
 void trl_drop_graphs(trl_handle* h) { destroy_graphs(h); }
 static void destroy_graphs(trl_handle* h) {
     for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
@@ -880,11 +910,11 @@ int trl_output_model(trl_handle* h, const char* path, uint32_t mtime) {
     return trl_write_model(path, ptr, h->mc.n_char, h->mc.n_frags, h->mc.frag, ptr[26], ptr[27], ptr[28], ptr[29], mtime);
 }
 int trl_trainer_set_theta(trl_trainer* t, const double* theta);
-// cNeuralNet::LoadModel + LoadScale (learning/NeuralNet.cpp:157-186): Caffe HDF5 weights + `_scale.txt`
-int trl_load_model(trl_handle* h, const char* h5_path, const char* scale_path) {
-    if (!h) return fail("trl_load_model: null handle");
-    if (!h->mc.has_net) return fail("trl_load_model: scene has no policy net");
-    if (h->trainer) return fail("trl_load_model: a trainer owns the policy weights (load before trl_trainer_create)");
+// cNeuralNet::LoadModel + LoadScale (learning/NeuralNet.cpp:157-186): reads Caffe HDF5 weights + `_scale.txt` and hands the 26 blobs and
+// the four offset / scale vectors (lengths checked against the scene's net) to use(blobs, counts, vec)
+extern "C++" {
+template <typename Use>
+static int read_model_files(trl_handle* h, const std::string& who, const char* h5_path, const char* scale_path, Use&& use) {
     try {
         H5Reader h5(h5_path);
         const auto& ds = h5.datasets();
@@ -893,7 +923,7 @@ int trl_load_model(trl_handle* h, const char* h5_path, const char* scale_path) {
         for (int l = 0; l < 13; ++l)
             for (int k = 0; k < 2; ++k) {
                 auto it = ds.find(std::string("/data/") + kNetLayers[l] + "/" + std::to_string(k));
-                if (it == ds.end()) return fail(std::string("trl_load_model: missing dataset for layer ") + kNetLayers[l]);
+                if (it == ds.end()) return fail(who + ": missing dataset for layer " + kNetLayers[l]);
                 blobs[2 * l + k] = it->second.data(); counts[2 * l + k] = (int64_t)it->second.size();
             }
         JValue sc = load_json(scale_path);
@@ -901,16 +931,90 @@ int trl_load_model(trl_handle* h, const char* h5_path, const char* scale_path) {
         std::vector<double> vec[4];
         for (int k = 0; k < 4; ++k) {
             const JValue* v = sc.get(keys[k]);
-            if (!v || v->type != JValue::Arr) return fail(std::string("trl_load_model: scale file lacks ") + keys[k]);
+            if (!v || v->type != JValue::Arr) return fail(who + ": scale file lacks " + keys[k]);
             for (auto& e : v->arr) vec[k].push_back(e.num);
             const size_t want = (size_t)(k < 2 ? h->mc.n_in : h->mc.n_out);
             if (vec[k].size() != want)
-                return fail(std::string("trl_load_model: ") + keys[k] + " has " + std::to_string(vec[k].size()) + " entries, the net needs " + std::to_string(want));
+                return fail(who + ": " + keys[k] + " has " + std::to_string(vec[k].size()) + " entries, the net needs " + std::to_string(want));
         }
-        return trl_set_weights(h, blobs, counts, 26, vec[0].data(), vec[1].data(), vec[2].data(), vec[3].data());
+        return use((const double* const*)blobs, (const int64_t*)counts, vec);
     } catch (const std::exception& e) {
         return fail(e.what());
     }
+}
+}  // extern "C++"
+int trl_load_model(trl_handle* h, const char* h5_path, const char* scale_path) {
+    if (!h) return fail("trl_load_model: null handle");
+    if (!h->mc.has_net) return fail("trl_load_model: scene has no policy net");
+    if (h->trainer) return fail("trl_load_model: a trainer owns the policy weights (load before trl_trainer_create)");
+    return read_model_files(h, "trl_load_model", h5_path, scale_path, [&](const double* const* blobs, const int64_t* counts, std::vector<double>* vec) {
+        return trl_set_weights(h, blobs, counts, 26, vec[0].data(), vec[1].data(), vec[2].data(), vec[3].data());
+    });
+}
+
+// every stream of the handle idle (the overlapped schedule leaves decisions and catch-up launches on the side streams, env groups on theirs)
+static int drain(trl_handle* h) {
+    CK(cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < h->lag; ++k) CK(cudaStreamSynchronize(h->side[k]));
+    for (int g = 0; g < kMaxGroups - 1; ++g)
+        if (h->group_stream[g]) CK(cudaStreamSynchronize(h->group_stream[g]));
+    return 0;
+}
+
+static bool slot_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxPolicySlots && !h->slot_blobs[slot].empty()); }
+
+int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* scale_path) {
+    if (!h) return fail("trl_load_policy: null handle");
+    if (slot < 1 || slot >= kMaxPolicySlots)
+        return fail("trl_load_policy: slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxPolicySlots - 1) + "; slot 0 is trl_load_model's)");
+    if (!h->mc.has_net) return fail("trl_load_policy: scene has no policy net");
+    if (h->mode != TRL_MODE_POLI_EVAL) return fail("trl_load_policy: policy slots are for evaluation handles (TRL_MODE_POLI_EVAL)");
+    if (h->trainer) return fail("trl_load_policy: a trainer is attached (it trains slot 0 in place; slots are for evaluation)");
+    if (!h->decide_v2) return fail("trl_load_policy: the TRL_DECIDE_V1 decision kernel has no policy slots");
+    if (!h5_path || !scale_path) return fail("trl_load_policy: null path");
+    return read_model_files(h, "trl_load_policy", h5_path, scale_path, [&](const double* const* blobs, const int64_t* counts, std::vector<double>* vec) {
+        const int64_t vcounts[4] = {h->mc.n_in, h->mc.n_in, h->mc.n_out, h->mc.n_out};
+        if (check_net_counts(h->mc, counts, vcounts)) return 1;
+        if (drain(h)) return 1;
+        if (!h->P.W) {      // first slot of this handle: per-env slots (all 0), weight table, sort scratch and chunk tables
+            PolicySlots& P = h->P;
+            int* env_slot = nullptr;
+            NetWeights* table = nullptr;
+            const size_t n = (size_t)h->n;
+            P.chunk_cap = h->n / 32 + kMaxPolicySlots;
+            CK(dalloc(h, &env_slot, n));
+            CK(dalloc(h, &table, (size_t)kMaxPolicySlots));
+            CK(dalloc(h, &P.sort_tmp, (size_t)h->lag * n));
+            CK(dalloc(h, &P.chunks, (size_t)h->lag * (1 + 3 * P.chunk_cap)));
+            CK(dalloc(h, &h->slot_stats, (size_t)kMaxPolicySlots * 4));
+            P.env_slot = env_slot; P.W = table;
+            h->env_slot_host.assign(n, 0);
+        }
+        const double* vecs[4] = {vec[0].data(), vec[1].data(), vec[2].data(), vec[3].data()};
+        if (upload_net(h, blobs, counts, vecs, vcounts, slot)) return 1;
+        h->slots_active = true;
+        h->slot_dirty = true;
+        return ensure_model(h) ? fail("trl_load_policy: slot table upload failed") : 0;
+    });
+}
+
+int trl_set_env_policy(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
+    if (!h) return fail("trl_set_env_policy: null handle");
+    if (n < 0 || n > h->n) return fail("trl_set_env_policy: env count out of range");
+    if (n > 0 && !slots) return fail("trl_set_env_policy: null slot list");
+    for (int k = 0; k < n; ++k) {
+        const int e = env_ids ? env_ids[k] : k;
+        if (e < 0 || e >= h->n) return fail("trl_set_env_policy: env id " + std::to_string(e) + " out of range");
+        if (slots[k] < 0 || slots[k] >= kMaxPolicySlots) return fail("trl_set_env_policy: slot " + std::to_string(slots[k]) + " out of range");
+        if (!slot_loaded(h, slots[k])) return fail("trl_set_env_policy: slot " + std::to_string(slots[k]) + " is empty (trl_load_policy first)");
+    }
+    if (!h->slots_active) return 0;      // only slot 0 exists, and every env is on it
+    std::vector<int> next = h->env_slot_host;
+    for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = slots[k];
+    if (drain(h)) return 1;
+    CK(cudaMemcpy((void*)h->P.env_slot, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
+    h->env_slot_host.swap(next);
+    return 0;
 }
 int trl_get_output_offset_scale(trl_handle* h, double* off, double* scale, int n);
 // the same for a scene pack, without a device (host-only: parses the pack and the controller tables); used to check the
@@ -1139,6 +1243,24 @@ int trl_eval_stats(trl_handle* h, int64_t* cycles, int64_t* episodes, double* av
     return 0;
 }
 
+int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+    if (!h) return fail("trl_eval_stats_slot: null handle");
+    if (slot < 0 || slot >= kMaxPolicySlots) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " out of range");
+    if (!slot_loaded(h, slot)) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " is empty");
+    if (!h->slots_active) return trl_eval_stats(h, cycles, episodes, avg_dist, env_steps);
+    double st[4];
+    launch_slot_stats(h->B, h->P.env_slot, h->slot_stats, h->stream);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(st, h->slot_stats + 4 * slot, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (cycles) *cycles = (int64_t)st[0];
+    if (episodes) *episodes = (int64_t)st[1];
+    if (env_steps) *env_steps = (int64_t)st[2];
+    if (avg_dist) *avg_dist = st[1] > 0 ? st[3] / st[1] : 0.0;
+    return 0;
+}
+
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {
     if (!h) return fail("trl_dist_log: null handle");
     int cnt = 0;
@@ -1291,11 +1413,7 @@ int trl_debug_decide(trl_handle* h, const int32_t* env_ids, int n, const double*
         }
     }
     if (ensure_model(h)) return fail("model upload failed");
-    // idle handle: the overlapped schedule leaves decisions and catch-up launches on the side streams and env groups on theirs
-    CK(cudaStreamSynchronize(h->stream));
-    for (int k = 0; k < h->lag; ++k) CK(cudaStreamSynchronize(h->side[k]));
-    for (int g = 0; g < kMaxGroups - 1; ++g)
-        if (h->group_stream[g]) CK(cudaStreamSynchronize(h->group_stream[g]));
+    if (drain(h)) return 1;
     if (poli_states) {
         const size_t S = (size_t)h->B.S;
         for (int k = 0; k < n;) {      // one copy per run of consecutive env ids
@@ -1342,7 +1460,7 @@ int trl_debug_time_decide(trl_handle* h, int n_pending, int iters, double* ms_av
 // kernel entry to stamp k (see trl_decide2.cuh: stamp()); conv_us / fc_us = event-timed durations of the two launches
 int trl_debug_fc_phases(trl_handle* h, int n_pending, double* out_ns16, double* conv_us, double* fc_us) {
     if (!h) return fail("trl_debug_fc_phases: null handle");
-    if (!h->decide_v2 || !h->mc.has_net) return fail("trl_debug_fc_phases: the batched decision path is not active");
+    if (!h->decide_v2 || !h->mc.has_net || h->slots_active) return fail("trl_debug_fc_phases: the single-policy batched decision path is not active");
     if (ensure_model(h)) return fail("model upload failed");
     n_pending = std::max(1, std::min(n_pending, h->n));
     unsigned long long* prof = nullptr;

@@ -115,7 +115,7 @@ extern "C" int trl_get_layer_state(trl_handle* h, int env, const char* layer_nam
         if (cudaMalloc((void**)&h->probe_dump, (size_t)L.total * 8) != cudaSuccess) return trl_fail("trl_get_layer_state: out of device memory");
         h->allocs.push_back(h->probe_dump);
     }
-    TRL_LAUNCH(trl_layer_probe_kernel, 1, 512, 0, h->stream, h->W, (const double*)(h->B.poli_state + (size_t)env * h->B.S), nc, nf, fr, h->probe_dump);
+    TRL_LAUNCH(trl_layer_probe_kernel, 1, 512, 0, h->stream, env_policy(h, env), (const double*)(h->B.poli_state + (size_t)env * h->B.S), nc, nf, fr, h->probe_dump);
     h->launches += 1;
     if (cudaGetLastError() != cudaSuccess || cudaStreamSynchronize(h->stream) != cudaSuccess) return trl_fail("trl_get_layer_state: probe kernel failed");
     const int n = std::min(hit->size, cap);

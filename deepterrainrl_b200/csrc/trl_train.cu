@@ -933,6 +933,7 @@ extern "C" {
 trl_trainer* trl_trainer_create(trl_handle* h, const double* p) {
     if (!h || !h->mc.has_net) { trl_fail("trl_trainer_create: the scene has no policy net"); return nullptr; }
     if (h->trainer) { trl_fail("trl_trainer_create: a trainer is already attached"); return nullptr; }
+    if (h->slots_active) { trl_fail("trl_trainer_create: the handle evaluates several policy slots (trl_load_policy); a trainer needs a single-policy handle"); return nullptr; }
     auto* t = new trl_trainer();
     t->h = h;
     Dev& d = t->d;

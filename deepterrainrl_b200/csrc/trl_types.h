@@ -167,6 +167,18 @@ inline NetWeights net_weights(const double* const* b, const double* in_off, cons
     return W;
 }
 
+// Policy slots of an evaluation handle (trl_load_policy): slot 0 is the handle's own net, slots 1 .. kMaxPolicySlots - 1 hold further
+// models of the same topology, each env is evaluated by the slot it is assigned to.  Only the slot build of the decision kernels
+// (trl_decide2.cuh) reads this; a handle with one policy never allocates it.
+constexpr int kMaxPolicySlots = 8;
+struct PolicySlots {
+    const int* env_slot;     // [n]  slot of each env
+    const NetWeights* W;     // [kMaxPolicySlots]  device table of the slots' weights (entries of empty slots are null)
+    int* sort_tmp;           // [lag][n]  copy of a pending list while it is regrouped by slot
+    int* chunks;             // [lag][1 + 3 * chunk_cap]  {number of chunks, then {slot, row0, rows} per 32-row FC chunk}
+    int chunk_cap;           // n / 32 + kMaxPolicySlots: every slot's ragged last chunk included
+};
+
 // Device buffers of one batch of environments.
 struct Buffers {
     int n;                 // number of envs

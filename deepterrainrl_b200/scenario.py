@@ -127,6 +127,7 @@ EXPORTS = [
     "trl_gather_tuples", "trl_gathered_blocks", "trl_gathered_fetch", "trl_gather_last_ms", "trl_trainer_add_gathered", "trl_trainer_broadcast",
     "trl_comm_broadcast_weights", "trl_comm_eval_stats", "trl_trainer_replica_spread", "trl_trainer_set_async",
     "trl_tc_split", "trl_tc_fc", "trl_tc_last_error", "trl_bench_last_span",
+    "trl_load_policy", "trl_set_env_policy", "trl_eval_stats_slot",
 ]
 
 
@@ -217,6 +218,26 @@ class BatchedScenario:
         """cNeuralNet::LoadModel + LoadScale from the reference's file formats."""
         scale_path = scale_path or (os.path.splitext(h5_path)[0] + "_scale.txt")
         self._ck(self.L.trl_load_model(self.h, h5_path.encode(), scale_path.encode()))
+
+    def LoadPolicy(self, slot, h5_path, scale_path=None):
+        """a further model (same net topology) into policy slot 1..7 of an evaluation scenario; envs move to it with SetEnvPolicy"""
+        scale_path = scale_path or (os.path.splitext(h5_path)[0] + "_scale.txt")
+        self._ck(self.L.trl_load_policy(self.h, int(slot), h5_path.encode(), scale_path.encode()))
+
+    def SetEnvPolicy(self, slots, env_ids=None):
+        """env_ids[k] (default: env k) is evaluated by the model in slots[k] from its next decision on"""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        if ids is not None and ids.size != s.size:
+            raise ValueError("SetEnvPolicy: one slot per env id")
+        self._ck(self.L.trl_set_env_policy(self.h, _p(ids), _p(s), int(s.size)))
+        if not hasattr(self, "_env_slot"):
+            self._env_slot = np.zeros(self.num_envs, np.int32)
+        self._env_slot[np.arange(s.size) if ids is None else ids] = s
+
+    def EnvPolicy(self):
+        """the slot of every env"""
+        return getattr(self, "_env_slot", np.zeros(self.num_envs, np.int32)).copy()
 
     def GetOutputOffsetScale(self):
         """cBaseControllerMACE::BuildNNOutputOffsetScale."""
@@ -368,13 +389,23 @@ class BatchedScenario:
     def GetNumEnvSteps(self):
         return self._stats()["steps"]
 
-    def GetDistLog(self):
+    def GetEvalStats(self, slot=0):
+        """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot`"""
+        c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
+        self._ck(self.L.trl_eval_stats_slot(self.h, int(slot), C.byref(c), C.byref(e), C.byref(a), C.byref(s)))
+        return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
+
+    def GetDistLog(self, slot=None):
+        """(distances, env ids) of the episodes logged so far; slot: only the entries of envs now on that policy slot"""
         d = C.c_void_p(); e = C.c_void_p(); n = C.c_int(0)
         self._ck(self.L.trl_dist_log(self.h, C.byref(d), C.byref(e), C.byref(n)))
         if n.value == 0:
             return np.zeros(0), np.zeros(0, np.int32)
         dist = np.ctypeslib.as_array(C.cast(d, C.POINTER(C.c_double)), (n.value,)).copy()
         env = np.ctypeslib.as_array(C.cast(e, C.POINTER(C.c_int32)), (n.value,)).copy()
+        if slot is not None:
+            keep = self.EnvPolicy()[env] == slot
+            dist, env = dist[keep], env[keep]
         return dist, env
 
 

@@ -162,6 +162,21 @@ int trl_output_model(trl_handle* h, const char* path, uint32_t mtime);
 int trl_write_model(const char* path, const double* const* blobs26, int n_char, int n_frags, int frag_size, const double* in_off,
                     const double* in_scale, const double* out_off, const double* out_scale, uint32_t mtime);
 int trl_get_output_offset_scale(trl_handle* h, double* offset, double* scale, int n_out);
+
+/* policy slots: one evaluation handle (TRL_MODE_POLI_EVAL) evaluates up to 8 models of the scene's net topology side by side, each env
+ * with the model of its slot.  Slot 0 is the handle's own policy (trl_create*, trl_load_model, trl_set_weights, trl_output_model);
+ * slots 1..7 start empty.  Results of an env do not depend on what else is in the batch: a mixed batch computes exactly what the
+ * single-policy handles would, env for env.
+ *   trl_load_policy      Caffe-HDF5 model + `_scale.txt` into slot 1..7; refused (handle unchanged) for another topology, an
+ *                        exploration handle, a handle with a trainer, and the TRL_DECIDE_V1 build.  trl_trainer_create refuses a
+ *                        handle with a loaded slot >= 1.
+ *   trl_set_env_policy   env_ids[k] (NULL: env k) -> slots[k] for k < n; every env starts on slot 0.  Refused, with nothing changed,
+ *                        for an env id or slot out of range or an empty slot.  Takes effect at the env's next decision, no reset.
+ *   trl_eval_stats_slot  trl_eval_stats over the envs now on `slot`.  trl_get_net_out / trl_get_layer_state / trl_debug_decide follow
+ *                        each env's slot; trl_dist_log entries carry env ids, so a caller splits them by slot itself. */
+int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* scale_json_path);
+int trl_set_env_policy(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n);
+int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
