@@ -63,6 +63,20 @@ std::vector<double> read_ctrl_params(const std::string& path, bool raptor) {
 
 }  // namespace
 
+TerrainFile read_terrain_file(const std::string& path) {
+    TerrainFile tf;
+    JValue t = load_json(path);
+    std::string type = t.string("Type", "flat");
+    if (type.empty()) type = "flat";
+    tf.type = index_of(kTerrainTypes, type, "terrain type");
+    if (const JValue* ps = t.get("Params"))
+        for (const JValue& s : ps->arr) {
+            for (int i = 0; i < 40; ++i) tf.params.push_back(s.number(kTerrainParams[i].name, kTerrainParams[i].dflt));
+            ++tf.n_sets;
+        }
+    return tf;
+}
+
 void build_scene_from_args(int argc, const char* const* argv, const std::string& root, ScenePack* out) {
     // CLI tokens first, then the arg file's, so the CLI wins on first-match lookup (optimizer/Main.cpp:19-32)
     ArgList args;
@@ -130,21 +144,13 @@ void build_scene_from_args(int argc, const char* const* argv, const std::string&
         for (int k = 0; k < ndof; ++k) { pose0[k] = pp->arr[k].num; vel0[k] = vv->arr[k].num; }
     }
 
-    int terrain_type = 0, n_sets = 0;
-    std::vector<double> tparams, tdefault(40);
+    std::vector<double> tdefault(40);
     for (int i = 0; i < 40; ++i) tdefault[i] = kTerrainParams[i].dflt;
     const std::string terrain_file = args.str("terrain_file", "");
-    if (!terrain_file.empty()) {
-        JValue t = load_json(join(root, terrain_file));
-        std::string type = t.string("Type", "flat");
-        if (type.empty()) type = "flat";
-        terrain_type = index_of(kTerrainTypes, type, "terrain type");
-        if (const JValue* ps = t.get("Params"))
-            for (const JValue& s : ps->arr) {
-                for (int i = 0; i < 40; ++i) tparams.push_back(s.number(kTerrainParams[i].name, kTerrainParams[i].dflt));
-                ++n_sets;
-            }
-    }
+    TerrainFile tf;
+    if (!terrain_file.empty()) tf = read_terrain_file(join(root, terrain_file));
+    const int terrain_type = tf.type, n_sets = tf.n_sets;
+    const std::vector<double>& tparams = tf.params;
 
     const bool has_init_x = args.has("char_init_pos_x");
     const std::string model = args.str("policy_model", "");

@@ -305,4 +305,14 @@ private:
 // arg file refer to (the DeepTerrainRL checkout).  Mirrors tools/pack_scene.py record for record.
 void build_scene_from_args(int argc, const char* const* argv, const std::string& root, ScenePack* out);
 
+// A terrain file (`-terrain_file`, cTerrainGen2D::LoadParams: {"Type": ..., "Params": [{...}, ...]}): the generator type and
+// n_sets parameter sets of 40 each, every parameter a file does not name at its cTerrainGen2D default.  Throws on an unknown type
+// or a malformed file.
+struct TerrainFile {
+    int type = 0;
+    int n_sets = 0;
+    std::vector<double> params;      // [n_sets][40]
+};
+TerrainFile read_terrain_file(const std::string& path);
+
 }  // namespace trl

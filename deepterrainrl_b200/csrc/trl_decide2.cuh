@@ -261,31 +261,33 @@ __global__ void __launch_bounds__(1024) trl_slot_sort_kernel(Buffers B, PolicySl
     }
 }
 
-// cycles / episodes / env-steps / episode-weighted distance of each policy slot's envs into out[kMaxPolicySlots][4], one slot after
-// the other with trl_stats_kernel's reduction (env_slot null: every env is on slot 0)
-__global__ void __launch_bounds__(1024) trl_slot_stats_kernel(Buffers B, const int* __restrict__ env_slot, double* __restrict__ out) {
+// cycles / episodes / env-steps / episode-weighted distance of the envs in one (policy slot, terrain slot) cell into
+// out[kMaxPolicySlots + 1][kMaxTerrainSlots + 1][4]; index kMaxPolicySlots / kMaxTerrainSlots = any slot.  One CTA per cell, each
+// with trl_stats_kernel's traversal and reduction order, so a cell's figures do not depend on the others (env_slot null: every env is
+// on policy slot 0; the terrain slot is the one the env's present ground came from)
+__global__ void __launch_bounds__(1024) trl_cell_stats_kernel(Buffers B, const int* __restrict__ env_slot, double* __restrict__ out) {
     __shared__ double red[4][32];
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
-    for (int p = 0; p < kMaxPolicySlots; ++p) {
-        double c = 0, e = 0, st = 0, ds = 0;
-        for (int env = threadIdx.x; env < B.n; env += blockDim.x) {
-            if ((env_slot ? env_slot[env] : 0) != p) continue;
-            const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
-            c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
-            e += ec;
-            st += (double)(((uint64_t)(uint32_t)B.i[(size_t)I_STEPS_HI * B.n + env] << 32) | (uint32_t)B.i[(size_t)I_STEPS_LO * B.n + env]);
-            ds += B.d[(size_t)D_AVG_DIST * B.n + env] * ec;
-        }
-        c = warp_sum_all(c); e = warp_sum_all(e); st = warp_sum_all(st); ds = warp_sum_all(ds);
-        if (l == 0) { red[0][w] = c; red[1][w] = e; red[2][w] = st; red[3][w] = ds; }
-        __syncthreads();
-        if (w == 0)
-            for (int k = 0; k < 4; ++k) {
-                const double v = warp_sum_all(l < nw ? red[k][l] : 0.0);
-                if (l == 0) out[4 * p + k] = v;
-            }
-        __syncthreads();
+    const int p = blockIdx.x / (kMaxTerrainSlots + 1), t = blockIdx.x % (kMaxTerrainSlots + 1);
+    const int* terrain_slot = B.i + (size_t)I_TERRAIN_SLOT * B.n;
+    double c = 0, e = 0, st = 0, ds = 0;
+    for (int env = threadIdx.x; env < B.n; env += blockDim.x) {
+        if (p < kMaxPolicySlots && (env_slot ? env_slot[env] : 0) != p) continue;
+        if (t < kMaxTerrainSlots && terrain_slot[env] != t) continue;
+        const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
+        c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
+        e += ec;
+        st += (double)(((uint64_t)(uint32_t)B.i[(size_t)I_STEPS_HI * B.n + env] << 32) | (uint32_t)B.i[(size_t)I_STEPS_LO * B.n + env]);
+        ds += B.d[(size_t)D_AVG_DIST * B.n + env] * ec;
     }
+    c = warp_sum_all(c); e = warp_sum_all(e); st = warp_sum_all(st); ds = warp_sum_all(ds);
+    if (l == 0) { red[0][w] = c; red[1][w] = e; red[2][w] = st; red[3][w] = ds; }
+    __syncthreads();
+    if (w == 0)
+        for (int k = 0; k < 4; ++k) {
+            const double v = warp_sum_all(l < nw ? red[k][l] : 0.0);
+            if (l == 0) out[4 * blockIdx.x + k] = v;
+        }
 }
 
 // the conv stage over the rows of a trainer minibatch (one cluster per row)
@@ -698,8 +700,8 @@ void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSetti
         TRL_LAUNCH_CLUSTER(kFcCluster, trl_decide_fc_slots_kernel, fc_clusters * kFcCluster, kFcThreads, decide_fc_smem_bytes(), st, B, P, ex, maps, smaps,
                            (const int*)tab, done_count, list, rearm);
 }
-void launch_slot_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st) {
-    TRL_LAUNCH(trl_slot_stats_kernel, 1, 1024, 0, st, B, env_slot, out);
+void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st) {
+    TRL_LAUNCH(trl_cell_stats_kernel, (kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1), 1024, 0, st, B, env_slot, out);
 }
 
 // the forward pass of a trainer minibatch through the same two kernels (trl_train.cu: enqueue_forward); act2 = [rows][5984] scratch the

@@ -55,7 +55,15 @@ struct trl_handle {
     std::vector<int> env_slot_host;
     trl::PolicySlots P{};                                    // device views (env_slot, weight table, sort scratch, chunk tables)
     trl::FcSlotMaps slot_maps{};
-    double* slot_stats = nullptr;                            // [kMaxPolicySlots][4]
+    // terrain slots (trl_load_terrain, any mode): slot 0 is mc.terrain_type / terrain_params, slots 1.. keep a terrain file's parameter
+    // sets, blended at terrain_lerp into terrain[] (the __constant__ table, uploaded with the model).  Until a slot >= 1 is loaded
+    // env_terrain_host is empty and every env is on slot 0 (the planes I_TERRAIN_SLOT / I_TERRAIN_SLOT_NEXT stay zero)
+    double terrain_lerp = 0.0;                                 // the handle's blend: -terrain_blend, then trl_set_terrain_lerp
+    trl::TerrainSlot terrain[trl::kMaxTerrainSlots] = {};
+    std::vector<double> terrain_sets[trl::kMaxTerrainSlots];   // [n_sets][40] of each loaded slot ([0] unused)
+    bool terrain_loaded[trl::kMaxTerrainSlots] = {};           // [0] unused
+    std::vector<int> env_terrain_host;                         // the assignment of every env (I_TERRAIN_SLOT_NEXT)
+    double* cell_stats = nullptr;                              // [kMaxPolicySlots + 1][kMaxTerrainSlots + 1][4] (trl_eval_stats_cell)
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
     bool use_graph = true;

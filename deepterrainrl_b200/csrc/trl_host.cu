@@ -19,7 +19,7 @@
 #include "trl_fcmaps.h"
 
 namespace trl {
-cudaError_t upload_model(const ModelConst& mc);
+cudaError_t upload_model(const ModelConst& mc, const TerrainSlot* terrain);
 size_t step_smem_bytes();
 cudaError_t configure_step_kernels();
 void launch_step(const Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
@@ -35,14 +35,32 @@ void launch_decide2(const Buffers& B, const NetWeights& W, const ExpSettings* ex
                     int fc_clusters, int list, int rearm, cudaStream_t st, int part);
 void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSettings* ex, const FcMaps& maps, const FcSlotMaps& smaps, double* act2,
                           int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part);
-void launch_slot_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
+void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
-cudaError_t upload_model(const trl::ModelConst& mc);
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_cg
+// the terrain-slot builds of the env-step kernels (trl_step_ts.cu, trl_step_ts_cg.cu); the emulator's trl / trl_cg builds are those
+#ifdef TRL_SIMT_EMU
+namespace trl_ts = trl;
+namespace trl_ts_cg = trl_cg;
+#else
+namespace trl_ts {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+void launch_reset(const trl::Buffers& B, const uint64_t* seeds, const int* env_ids, int count, int reseed, cudaStream_t st);
+void launch_terrain(const trl::Buffers& B, double lookahead, cudaStream_t st);
+}  // namespace trl_ts
+namespace trl_ts_cg {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+}  // namespace trl_ts_cg
+#endif
 
 
 using namespace trl;
@@ -51,9 +69,11 @@ using namespace trl;
 struct trl_handle;
 static const trl_handle* g_model_owner = nullptr;    // whose ModelConst currently sits in the __constant__ copies
 static int g_device = -1;                             // the one device this process drives (set by the first handle)
-static cudaError_t upload_model_all(const ModelConst& mc) {
-    cudaError_t e = trl::upload_model(mc);
-    return e != cudaSuccess ? e : trl_cg::upload_model(mc);
+static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain) {
+    cudaError_t e = trl::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_cg::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_ts::upload_model(mc, terrain);
+    return e != cudaSuccess ? e : trl_ts_cg::upload_model(mc, terrain);
 }
 
 static thread_local std::string g_err;
@@ -85,7 +105,9 @@ static int ensure_model_only(trl_handle* h) {
     // that was created first; a handle on another device is refused at creation (create_common)
     if (g_model_owner == h) return 0;
     if (cudaDeviceSynchronize() != cudaSuccess) return 1;
-    if (upload_model_all(h->mc) != cudaSuccess) return 1;
+    h->terrain[0].type = h->mc.terrain_type;      // slot 0 of the terrain table is the scene's own terrain
+    std::memcpy(h->terrain[0].params, h->mc.terrain_params, sizeof(h->mc.terrain_params));
+    if (upload_model_all(h->mc, h->terrain) != cudaSuccess) return 1;
     g_model_owner = h;
     return 0;
 }
@@ -94,6 +116,19 @@ int trl_reupload_model(trl_handle* h) {
     if (!h) return fail("trl_reupload_model: null handle");
     g_model_owner = nullptr;
     return ensure_model(h) ? fail("model upload failed") : 0;
+}
+
+// cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272): n_sets parameter sets [n_sets][40] blended at
+// `lerp` (clamped to the sets there are); no set = the generator's defaults
+static void blend_terrain(const double* sets, int n_sets, const double* dflt, double lerp, double* out) {
+    if (n_sets <= 0) {
+        for (int i = 0; i < kTerrainParams; ++i) out[i] = dflt[i];
+        return;
+    }
+    lerp = std::min(std::max(lerp, 0.0), n_sets - 1.0);
+    const int i0 = (int)lerp, i1 = std::min(i0 + 1, n_sets - 1);
+    lerp -= i0;
+    for (int i = 0; i < kTerrainParams; ++i) out[i] = (1 - lerp) * sets[i0 * kTerrainParams + i] + lerp * sets[i1 * kTerrainParams + i];
 }
 
 template <typename T>
@@ -311,15 +346,8 @@ static int fill_model(trl_handle* h, uint64_t rng_seed) {
     const auto& v0 = s.f64("vel0");
     for (int k = 0; k < m.ndof; ++k) { m.pose0[k] = p0[k]; m.vel0[k] = v0[k]; }
     // cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272)
-    const auto& tp = s.f64("terrain_params");
-    const auto& td = s.f64("terrain_default_params");
-    if (n_sets == 0) for (int i = 0; i < kTerrainParams; ++i) m.terrain_params[i] = td[i];
-    else {
-        double lerp = std::min(std::max(mf[3], 0.0), n_sets - 1.0);
-        int i0 = (int)lerp, i1 = std::min(i0 + 1, n_sets - 1);
-        lerp -= i0;
-        for (int i = 0; i < kTerrainParams; ++i) m.terrain_params[i] = (1 - lerp) * tp[i0 * kTerrainParams + i] + lerp * tp[i1 * kTerrainParams + i];
-    }
+    blend_terrain(s.f64("terrain_params").data(), n_sets, s.f64("terrain_default_params").data(), mf[3], m.terrain_params);
+    h->terrain_lerp = mf[3];
     {
         const char* vc = std::getenv("TRL_VERTEX_CONTACTS");
         m.phys = PhysParams{2.0e5, 2.0e3, 0.81, 0.01, 0.00025, 2.0e4, 20.0, (vc && vc[0] == '1') ? 1 : 0};
@@ -470,6 +498,24 @@ static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, 
     else if (part & 1)
         launch_decide(h->B, h->W, h->d_ex, h->done_count, h->decide_grid, list, rearm, st);
 }
+// the env-step launches of a handle: the terrain-slot builds once a terrain slot is loaded (trl_load_terrain), else the plain ones
+static bool terrain_slots(const trl_handle* h) { return !h->env_terrain_host.empty(); }
+static void step_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1) {
+    if (terrain_slots(h)) trl_ts::launch_step(h->B, step, flags, lists, st, group, n_groups);
+    else launch_step(h->B, step, flags, lists, st, group, n_groups);
+}
+static void catchup_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st) {
+    if (terrain_slots(h)) trl_ts_cg::launch_step(h->B, step, flags, lists, st);
+    else trl_cg::launch_step(h->B, step, flags, lists, st);
+}
+static void terrain_launch(const trl_handle* h, cudaStream_t st) {
+    if (terrain_slots(h)) trl_ts::launch_terrain(h->B, 0.5, st);
+    else launch_terrain(h->B, 0.5, st);
+}
+static void reset_launch(const trl_handle* h, const uint64_t* seeds, const int* env_ids, int count, int reseed) {
+    if (terrain_slots(h)) trl_ts::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+    else launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+}
 static int num_decide_launches(const trl_handle* h) { return h->decide_v2 ? (h->slots_active ? 3 : 2) : 1; }
 
 void trl_drop_graphs(trl_handle* h) { destroy_graphs(h); }
@@ -521,13 +567,13 @@ static void enqueue_update(trl_handle* h, double dt, bool overlap, Timeline* tl 
     cudaStream_t A = h->stream;
 #define TL_OPEN(st, k, i) do { if (tl) tl->open(st, k, i); } while (0)
 #define TL_CLOSE(st) do { if (tl) tl->close(st); } while (0)
-    TL_OPEN(A, 0, 0); launch_terrain(h->B, 0.5, A); TL_CLOSE(A);
+    TL_OPEN(A, 0, 0); terrain_launch(h, A); TL_CLOSE(A);
     if (!overlap) {
         for (int i = 0; i < ns; ++i) {
-            TL_OPEN(A, 1, i); launch_step(h->B, step, i == 0 ? 2 : 3, 0, A); TL_CLOSE(A);
+            TL_OPEN(A, 1, i); step_launch(h, step, i == 0 ? 2 : 3, 0, A); TL_CLOSE(A);
             TL_OPEN(A, 2, i); enqueue_decide(h, 0, 1, A, 1); TL_CLOSE(A); TL_OPEN(A, 4, i); enqueue_decide(h, 0, 1, A, 2); TL_CLOSE(A);
         }
-        TL_OPEN(A, 1, ns); launch_step(h->B, step, 1 | 4, 0, A); TL_CLOSE(A);
+        TL_OPEN(A, 1, ns); step_launch(h, step, 1 | 4, 0, A); TL_CLOSE(A);
         return;
     }
     // Overlapped schedule, `lag` env-steps deep.  Main stream: T S_0 S_1 S_2 ... S_{ns-1} S_end back to back.  The envs that reach a
@@ -555,7 +601,7 @@ static void enqueue_update(trl_handle* h, double dt, bool overlap, Timeline* tl 
     if (G > 1) { cudaEventRecord(ev_t, A); for (int g = 1; g < G; ++g) cudaStreamWaitEvent(stream_of(g), ev_t, 0); }
     for (int g = 0; g < G; ++g) {
         cudaStream_t M = stream_of(g);
-        TL_OPEN(M, 1, 0); launch_step(h->B, step, 2, lists_of(0, 0, 0), M, g, G); TL_CLOSE(M);
+        TL_OPEN(M, 1, 0); step_launch(h, step, 2, lists_of(0, 0, 0), M, g, G); TL_CLOSE(M);
         cudaEventRecord(ev_s[g], M);
     }
     for (int i = 1; i < ns; ++i) {
@@ -565,12 +611,12 @@ static void enqueue_update(trl_handle* h, double dt, bool overlap, Timeline* tl 
         for (int g = 0; g < G; ++g) cudaStreamWaitEvent(X, ev_s[l * G + g], 0);
         TL_OPEN(X, 2, l); enqueue_decide(h, l % nl, 0, X, 1, slot); TL_CLOSE(X); TL_OPEN(X, 4, l); enqueue_decide(h, l % nl, 0, X, 2, slot); TL_CLOSE(X);
         const int reps = std::min(lag, ns - 1 - l);     // equivalents l + 1 .. l + reps of the main launches; S_end is never caught up
-        TL_OPEN(X, 3, l); trl_cg::launch_step(h->B, step, 1 | 2 | 16, lists_of(l + 1, l, reps), X); TL_CLOSE(X);
+        TL_OPEN(X, 3, l); catchup_launch(h, step, 1 | 2 | 16, lists_of(l + 1, l, reps), X); TL_CLOSE(X);
         cudaEventRecord(ev_c[l], X);
         for (int g = 0; g < G; ++g) {
             cudaStream_t M = stream_of(g);
             if (i >= nl) cudaStreamWaitEvent(M, ev_c[i - nl], 0);
-            TL_OPEN(M, 1, i); launch_step(h->B, step, 1 | 2 | 8, lists_of(i, i, 0), M, g, G); TL_CLOSE(M);
+            TL_OPEN(M, 1, i); step_launch(h, step, 1 | 2 | 8, lists_of(i, i, 0), M, g, G); TL_CLOSE(M);
             cudaEventRecord(ev_s[i * G + g], M);
         }
     }
@@ -583,7 +629,7 @@ static void enqueue_update(trl_handle* h, double dt, bool overlap, Timeline* tl 
     }
     for (int l = std::max(0, ns - nl); l < ns; ++l) cudaStreamWaitEvent(A, ev_c[l], 0);     // every side stream joins here
     for (int g = 1; g < G; ++g) cudaStreamWaitEvent(A, ev_s[(ns - 1) * G + g], 0);          // and every group stream
-    TL_OPEN(A, 1, ns); launch_step(h->B, step, 1 | 4, 0, A); TL_CLOSE(A);
+    TL_OPEN(A, 1, ns); step_launch(h, step, 1 | 4, 0, A); TL_CLOSE(A);
 #undef TL_OPEN
 #undef TL_CLOSE
 }
@@ -677,7 +723,9 @@ static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mo
     };
     g_model_owner = nullptr;
     if (ensure_model(h)) return bail("upload_model failed");
-    if (!ck(configure_step_kernels(), "configure_step_kernels") || !ck(trl_cg::configure_step_kernels(), "configure_step_kernels")) return bail("");
+    if (!ck(configure_step_kernels(), "configure_step_kernels") || !ck(trl_cg::configure_step_kernels(), "configure_step_kernels") ||
+        !ck(trl_ts::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ts_cg::configure_step_kernels(), "configure_step_kernels"))
+        return bail("");
     if (!ck(configure_decide_kernel(), "configure_decide_kernel")) return bail("");
     if (!ck(configure_decide2_kernels(), "configure_decide2_kernels")) return bail("");
     {
@@ -695,7 +743,7 @@ static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mo
     // fixed-size exchange block (trl_gather_tuples) drains the queue
     B.tuple_cap = std::max(4096, 2 * num_envs);
     B.dist_cap = std::max(65536, 16 * num_envs);
-    bool ok = ck(dalloc(h, &B.d, (size_t)D_NUM_FIELDS * n), "alloc d") && ck(dalloc(h, &B.i, (size_t)I_NUM_FIELDS * n), "alloc i") &&
+    bool ok = ck(dalloc(h, &B.d, (size_t)D_NUM_FIELDS * n), "alloc d") && ck(dalloc(h, &B.i, (size_t)I_NUM_PLANES * n), "alloc i") &&
               ck(dalloc(h, &B.terrain, n * 2 * kTerrainCap), "alloc terrain") && ck(dalloc(h, &B.poli_state, n * B.S), "alloc poli") &&
               ck(dalloc(h, &B.net_out, n * kMaxNetOut), "alloc net_out") && ck(dalloc(h, &B.tuple_sbeg, n * B.S), "alloc sbeg") &&
               ck(dalloc(h, &B.tuple_action, n * kNumParams), "alloc action") && ck(dalloc(h, &B.com_stash, 2 * n), "alloc com") &&
@@ -767,7 +815,7 @@ int trl_seed_terrain(trl_handle* h, const uint64_t* seeds, int n) {
     }
     cudaError_t e = cudaMemsetAsync(h->B.pending_count, 0, kMaxLists * 4, h->stream);
     if (e == cudaSuccess) {
-        launch_reset(h->B, d_seeds, nullptr, h->n, 1, h->stream);
+        reset_launch(h, d_seeds, nullptr, h->n, 1);
         h->launches += 1;
         e = cudaGetLastError();
     }
@@ -792,7 +840,7 @@ int trl_reset(trl_handle* h, const int32_t* env_ids, int n) {
         cudaError_t e = cudaMemcpyAsync(d_ids, env_ids, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream);
         if (e != cudaSuccess) { cudaFree(d_ids); return fail(std::string("trl_reset: ") + cudaGetErrorString(e)); }
     }
-    launch_reset(h->B, nullptr, d_ids, count, 0, h->stream);
+    reset_launch(h, nullptr, d_ids, count, 0);
     h->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
@@ -832,9 +880,9 @@ int trl_update(trl_handle* h, double dt) {
 int trl_env_step(trl_handle* h, double step) {
     if (!h) return fail("trl_env_step: null handle");
     if (ensure_model(h)) return fail("model upload failed");
-    launch_step(h->B, step, 2, 0, h->stream);
+    step_launch(h, step, 2, 0, h->stream);
     enqueue_decide(h, 0, 1, h->stream);
-    launch_step(h->B, step, 1, 0, h->stream);
+    step_launch(h, step, 1, 0, h->stream);
     h->launches += 2 + num_decide_launches(h);
     CK(cudaGetLastError());
     return 0;
@@ -986,7 +1034,6 @@ int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* sc
             CK(dalloc(h, &table, (size_t)kMaxPolicySlots));
             CK(dalloc(h, &P.sort_tmp, (size_t)h->lag * n));
             CK(dalloc(h, &P.chunks, (size_t)h->lag * (1 + 3 * P.chunk_cap)));
-            CK(dalloc(h, &h->slot_stats, (size_t)kMaxPolicySlots * 4));
             P.env_slot = env_slot; P.W = table;
             h->env_slot_host.assign(n, 0);
         }
@@ -1014,6 +1061,63 @@ int trl_set_env_policy(trl_handle* h, const int32_t* env_ids, const int32_t* slo
     if (drain(h)) return 1;
     CK(cudaMemcpy((void*)h->P.env_slot, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
     h->env_slot_host.swap(next);
+    return 0;
+}
+
+static bool terrain_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxTerrainSlots && h->terrain_loaded[slot]); }
+
+int trl_load_terrain(trl_handle* h, int slot, const char* terrain_json_path) {
+    if (!h) return fail("trl_load_terrain: null handle");
+    if (slot < 1 || slot >= kMaxTerrainSlots)
+        return fail("trl_load_terrain: slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxTerrainSlots - 1) + "; slot 0 is the scene's terrain)");
+    if (!terrain_json_path) return fail("trl_load_terrain: null path");
+    TerrainFile tf;
+    try {
+        tf = read_terrain_file(terrain_json_path);
+    } catch (const std::exception& e) {
+        return fail(std::string("trl_load_terrain: ") + e.what());
+    }
+    TerrainSlot ts{};
+    ts.type = tf.type;
+    blend_terrain(tf.params.data(), tf.n_sets, h->scene.f64("terrain_default_params").data(), h->terrain_lerp, ts.params);
+    if (drain(h)) return 1;
+    if (h->env_terrain_host.empty()) {     // first slot: from now on the step launches run the terrain-slot build
+        h->env_terrain_host.assign((size_t)h->n, 0);
+        destroy_graphs(h);
+    }
+    h->terrain_sets[slot] = std::move(tf.params);
+    h->terrain_loaded[slot] = true;
+    h->terrain[slot] = ts;
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail("trl_load_terrain: terrain table upload failed") : 0;
+}
+
+int trl_set_env_terrain(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
+    if (!h) return fail("trl_set_env_terrain: null handle");
+    if (n < 0 || n > h->n) return fail("trl_set_env_terrain: env count out of range");
+    if (n > 0 && !slots) return fail("trl_set_env_terrain: null slot list");
+    for (int k = 0; k < n; ++k) {
+        const int e = env_ids ? env_ids[k] : k;
+        if (e < 0 || e >= h->n) return fail("trl_set_env_terrain: env id " + std::to_string(e) + " out of range");
+        if (slots[k] < 0 || slots[k] >= kMaxTerrainSlots) return fail("trl_set_env_terrain: slot " + std::to_string(slots[k]) + " out of range");
+        if (!terrain_loaded(h, slots[k])) return fail("trl_set_env_terrain: slot " + std::to_string(slots[k]) + " is empty (trl_load_terrain first)");
+    }
+    if (h->env_terrain_host.empty()) return 0;      // only slot 0 exists, and every env is on it
+    std::vector<int> next = h->env_terrain_host;
+    for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = slots[k];
+    if (drain(h)) return 1;
+    CK(cudaMemcpy(h->B.i + (size_t)I_TERRAIN_SLOT_NEXT * h->n, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
+    h->env_terrain_host.swap(next);
+    return 0;
+}
+
+int trl_env_terrain(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
+    if (!h) return fail("trl_env_terrain: null handle");
+    if (n < 0 || n > h->n) return fail("trl_env_terrain: env count out of range");
+    if (drain(h)) return 1;
+    const size_t N = (size_t)h->n;
+    if (current && n > 0) CK(cudaMemcpy(current, h->B.i + (size_t)I_TERRAIN_SLOT * N, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (assigned && n > 0) CK(cudaMemcpy(assigned, h->B.i + (size_t)I_TERRAIN_SLOT_NEXT * N, (size_t)n * 4, cudaMemcpyDeviceToHost));
     return 0;
 }
 int trl_get_output_offset_scale(trl_handle* h, double* off, double* scale, int n);
@@ -1064,24 +1168,29 @@ int trl_get_output_offset_scale(trl_handle* h, double* off, double* scale, int n
 
 // cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272), as cScenarioTrain::UpdateSceneCurriculum calls it
 // (scenarios/ScenarioTrain.cpp:412-416): blends the scene's terrain parameter sets; segments generated from now on use the
-// blend (cGroundVar2D::SetTerrainParams), existing terrain stays.
+// blend (cGroundVar2D::SetTerrainParams), existing terrain stays.  Every loaded terrain slot is re-blended at the same `lerp`.
 int trl_set_terrain_lerp(trl_handle* h, double lerp) {
     if (!h) return fail("trl_set_terrain_lerp: null handle");
+    h->terrain_lerp = lerp;
     const auto& tp = h->scene.f64("terrain_params");
+    const auto& td = h->scene.f64("terrain_default_params");
     const int n_sets = (int)(tp.size() / kTerrainParams);
-    if (n_sets <= 0) return 0;
-    lerp = std::min(std::max(lerp, 0.0), n_sets - 1.0);
-    const int i0 = (int)lerp, i1 = std::min(i0 + 1, n_sets - 1);
-    lerp -= i0;
-    double blended[kTerrainParams];
+    double blended[kMaxTerrainSlots][kTerrainParams];
     bool same = true;
-    for (int i = 0; i < kTerrainParams; ++i) {
-        blended[i] = (1 - lerp) * tp[i0 * kTerrainParams + i] + lerp * tp[i1 * kTerrainParams + i];
-        same = same && blended[i] == h->mc.terrain_params[i];
+    if (n_sets > 0) {       // a scene without parameter sets keeps its defaults whatever the blend
+        blend_terrain(tp.data(), n_sets, td.data(), lerp, blended[0]);
+        same = std::equal(blended[0], blended[0] + kTerrainParams, h->mc.terrain_params);
+    }
+    for (int s = 1; s < kMaxTerrainSlots; ++s) {
+        if (!h->terrain_loaded[s]) continue;
+        blend_terrain(h->terrain_sets[s].data(), (int)(h->terrain_sets[s].size() / kTerrainParams), td.data(), lerp, blended[s]);
+        same = same && std::equal(blended[s], blended[s] + kTerrainParams, h->terrain[s].params);
     }
     if (same) return 0;      // cScenarioTrain calls this after every trainer step; an unchanged blend must not drain the device
-    CK(cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < kTerrainParams; ++i) h->mc.terrain_params[i] = blended[i];
+    if (drain(h)) return 1;
+    if (n_sets > 0) std::memcpy(h->mc.terrain_params, blended[0], sizeof(blended[0]));
+    for (int s = 1; s < kMaxTerrainSlots; ++s)
+        if (h->terrain_loaded[s]) std::memcpy(h->terrain[s].params, blended[s], sizeof(blended[s]));
     g_model_owner = nullptr;
     if (ensure_model(h)) return fail("model upload failed");
     return 0;
@@ -1243,22 +1352,40 @@ int trl_eval_stats(trl_handle* h, int64_t* cycles, int64_t* episodes, double* av
     return 0;
 }
 
-int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
-    if (!h) return fail("trl_eval_stats_slot: null handle");
-    if (slot < 0 || slot >= kMaxPolicySlots) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " out of range");
-    if (!slot_loaded(h, slot)) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " is empty");
-    if (!h->slots_active) return trl_eval_stats(h, cycles, episodes, avg_dist, env_steps);
+// trl_eval_stats over the envs of one (policy slot, terrain slot) cell, -1 = any slot.  A cell that holds every env is trl_eval_stats
+// itself; the others come from trl_cell_stats_kernel
+static int eval_stats_cell(trl_handle* h, const char* who, int policy_slot, int terrain_slot, int64_t* cycles, int64_t* episodes,
+                           double* avg_dist, int64_t* env_steps) {
+    if (!h) return fail(std::string(who) + ": null handle");
+    if (policy_slot < -1 || policy_slot >= kMaxPolicySlots) return fail(std::string(who) + ": policy slot " + std::to_string(policy_slot) + " out of range");
+    if (policy_slot >= 0 && !slot_loaded(h, policy_slot)) return fail(std::string(who) + ": policy slot " + std::to_string(policy_slot) + " is empty");
+    if (terrain_slot < -1 || terrain_slot >= kMaxTerrainSlots) return fail(std::string(who) + ": terrain slot " + std::to_string(terrain_slot) + " out of range");
+    if (terrain_slot >= 0 && !terrain_loaded(h, terrain_slot)) return fail(std::string(who) + ": terrain slot " + std::to_string(terrain_slot) + " is empty");
+    const bool any_p = policy_slot < 0 || !h->slots_active, any_t = terrain_slot < 0 || h->env_terrain_host.empty();
+    if (any_p && any_t) return trl_eval_stats(h, cycles, episodes, avg_dist, env_steps);
+    if (!h->cell_stats) CK(dalloc(h, &h->cell_stats, (size_t)(kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1) * 4));
+    const int cell = (any_p ? kMaxPolicySlots : policy_slot) * (kMaxTerrainSlots + 1) + (any_t ? kMaxTerrainSlots : terrain_slot);
     double st[4];
-    launch_slot_stats(h->B, h->P.env_slot, h->slot_stats, h->stream);
+    launch_cell_stats(h->B, h->slots_active ? h->P.env_slot : nullptr, h->cell_stats, h->stream);
     h->launches += 1;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(st, h->slot_stats + 4 * slot, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(st, h->cell_stats + 4 * cell, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (cycles) *cycles = (int64_t)st[0];
     if (episodes) *episodes = (int64_t)st[1];
     if (env_steps) *env_steps = (int64_t)st[2];
     if (avg_dist) *avg_dist = st[1] > 0 ? st[3] / st[1] : 0.0;
     return 0;
+}
+
+int trl_eval_stats_cell(trl_handle* h, int policy_slot, int terrain_slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+    return eval_stats_cell(h, "trl_eval_stats_cell", policy_slot, terrain_slot, cycles, episodes, avg_dist, env_steps);
+}
+
+int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+    if (!h) return fail("trl_eval_stats_slot: null handle");
+    if (slot < 0 || slot >= kMaxPolicySlots) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " out of range");
+    return eval_stats_cell(h, "trl_eval_stats_slot", slot, -1, cycles, episodes, avg_dist, env_steps);
 }
 
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {
@@ -1645,17 +1772,17 @@ static int update_timed_impl(trl_handle* h, double dt, double* step_ms, int* ste
     std::vector<cudaEvent_t> ev(2 * (2 * ns + 1));
     for (auto& e : ev) CK(cudaEventCreate(&e));
     int k = 0;
-    launch_terrain(h->B, 0.5, h->stream);
+    terrain_launch(h, h->stream);
     for (int i = 0; i < ns; ++i) {
         CK(cudaEventRecord(ev[k++], h->stream));
-        launch_step(h->B, step, i == 0 ? 2 : 3, 0, h->stream);
+        step_launch(h, step, i == 0 ? 2 : 3, 0, h->stream);
         CK(cudaEventRecord(ev[k++], h->stream));
         CK(cudaEventRecord(ev[k++], h->stream));
         enqueue_decide(h, 0, 1, h->stream);
         CK(cudaEventRecord(ev[k++], h->stream));
     }
     CK(cudaEventRecord(ev[k++], h->stream));
-    launch_step(h->B, step, 1 | 4, 0, h->stream);
+    step_launch(h, step, 1 | 4, 0, h->stream);
     CK(cudaEventRecord(ev[k++], h->stream));
     CK(cudaStreamSynchronize(h->stream));
     CK(cudaGetLastError());

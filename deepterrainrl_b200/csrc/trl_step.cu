@@ -36,7 +36,15 @@
 // every global load bypasses L1.  The cg build serves the catch-up launches of the overlapped schedule: they read env state the
 // decision kernel has just written, while step CTAs running on the same SM may already have pulled the neighbouring envs'
 // words of the same 32-byte sectors into that SM's L1.
-#if defined(TRL_CG_VARIANT)
+// Terrain slots (trl_load_terrain) are served by two more builds, trl_step_ts.cu (namespace trl_ts) and trl_step_ts_cg.cu (trl_ts_cg),
+// compiled with TRL_TERRAIN_SLOTS_VARIANT: their envs generate their ground from their own slot of c_terrain.  The builds without it
+// generate from c_model's terrain, so a handle without terrain slots runs the same kernels as before slots existed.  The emulator
+// (tests/simt) compiles only trl_step.cu / trl_step_cg.cu and always with slots, which computes the same for a handle without any.
+#if defined(TRL_TERRAIN_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
+#define TRL_IMPL_NS trl_ts_cg
+#elif defined(TRL_TERRAIN_SLOTS_VARIANT)
+#define TRL_IMPL_NS trl_ts
+#elif defined(TRL_CG_VARIANT)
 #define TRL_IMPL_NS trl_cg
 #else
 #define TRL_IMPL_NS trl
@@ -44,8 +52,14 @@
 
 namespace TRL_IMPL_NS {
 using namespace trl;
+#if defined(TRL_TERRAIN_SLOTS_VARIANT) || defined(TRL_SIMT_EMU)
+constexpr bool kTerrainSlots = true;
+#else
+constexpr bool kTerrainSlots = false;
+#endif
 
 __constant__ ModelConst c_model;
+__constant__ TerrainSlot c_terrain[kMaxTerrainSlots];    // slot 0 = c_model's terrain_type / terrain_params (trl_types.h: TerrainSlot)
 // character-type branches: a run-time constant of the scene (the raptor's controller differs from the dog's / goat's); an experiment
 // build can fix it at compile time (-DTRL_FIXED_CHAR=0 dog / goat, 2 raptor) to see what the unused branches cost
 #ifdef TRL_FIXED_CHAR
@@ -403,6 +417,9 @@ __device__ void store_ground(Lane& L, const GroundView& g) {
     L.i(I_SEG_FLIP) = g.flip;
     L.i(I_TERRAIN_RNG) = (int)g.rng_state;
 }
+
+// the terrain slot the env's present ground comes from; I_TERRAIN_SLOT is not a staged field, so this reads the plane itself
+__device__ __forceinline__ const TerrainSlot& env_terrain(const Lane& L) { return c_terrain[L.I[(size_t)I_TERRAIN_SLOT * L.n + L.env]]; }
 
 __device__ CounterRng load_rng(Lane& L) {
     CounterRng r;
@@ -1230,9 +1247,15 @@ __device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B
         L.d(D_FALL_DIST_CNT) = 5.0; L.d(D_PREV_CHECK_X) = e.ox; L.d(D_PREV_CHECK_Y) = e.oy;
         L.i(I_FAIL_FALL_DIST) = 0; L.d(D_FALL_CONTACT_CNT) = 0.1; L.d(D_SUM_FALL) = 0.0;
         // ResetGround + InitCharacterPos
+        int slot = 0;
+        if constexpr (kTerrainSlots) {      // the terrain slot assigned to the env (trl_set_env_terrain) becomes its current one
+            slot = L.I[(size_t)I_TERRAIN_SLOT_NEXT * L.n + L.env];
+            L.I[(size_t)I_TERRAIN_SLOT * L.n + L.env] = slot;
+        }
         GroundView g = load_ground(L, B);
         g.n[0] = g.n[1] = 0; g.flip = 0;
-        g.update(-11.0, 9.0, m.terrain_type, m.terrain_params, 20.0);
+        if constexpr (kTerrainSlots) g.update(-11.0, 9.0, c_terrain[slot].type, c_terrain[slot].params, 20.0);
+        else g.update(-11.0, 9.0, m.terrain_type, m.terrain_params, 20.0);
         if (m.has_init_x) newx = m.init_x;
         newy = e.oy + g.sample(newx);
         store_ground(L, g);
@@ -1463,7 +1486,11 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
             double bmin = e.ox - 2.0, bmax = e.ox + 10.0 + 1.0;
             bool need = !(bmax < g.seg_max_x(smax) && bmin > g.seg_min_x(smin));
             if (need) {
-                if (lane == 0) { g.update(bmin, bmax, m.terrain_type, m.terrain_params, 20.0); store_ground(L, g); }
+                if (lane == 0) {
+                    if constexpr (kTerrainSlots) { const TerrainSlot& ts = env_terrain(L); g.update(bmin, bmax, ts.type, ts.params, 20.0); }
+                    else g.update(bmin, bmax, m.terrain_type, m.terrain_params, 20.0);
+                    store_ground(L, g);
+                }
                 __syncwarp();
                 g = load_ground(L, B);
             }
@@ -1579,14 +1606,18 @@ trl_reset_kernel(Buffers B, const uint64_t* terrain_seeds, const int* env_ids, i
 __global__ void trl_terrain_kernel(Buffers B, double lookahead) {
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= B.n) return;
-    const ModelConst& m = c_model;
     Lane L{nullptr, env, B.n, B.d, B.i};
     const double x = L.d(D_Q);
     GroundView g = load_ground(L, B);
     const int smin = g.seg_id(0), smax = g.seg_id(1);
     const double bmin = x - 2.0, bmax = x + 10.0 + 1.0 + lookahead;
     if (bmax < g.seg_max_x(smax) && bmin > g.seg_min_x(smin)) return;
-    g.update(bmin, bmax, m.terrain_type, m.terrain_params, 20.0);
+    if constexpr (kTerrainSlots) {
+        const TerrainSlot& ts = env_terrain(L);
+        g.update(bmin, bmax, ts.type, ts.params, 20.0);
+    } else {
+        g.update(bmin, bmax, c_model.terrain_type, c_model.terrain_params, 20.0);
+    }
     store_ground(L, g);
 }
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st) {
@@ -1621,8 +1652,9 @@ __global__ void trl_stats_kernel(Buffers B, double* out) {
 void launch_stats(const Buffers& B, double* out, cudaStream_t st) { TRL_LAUNCH(trl_stats_kernel, 1, 1024, 0, st, B, out); }
 
 // ---- host-side launch helpers (called from trl_host.cu)
-cudaError_t upload_model(const ModelConst& mc) {
+cudaError_t upload_model(const ModelConst& mc, const TerrainSlot* terrain) {
     cudaError_t e = cudaMemcpyToSymbol(c_model, &mc, sizeof(ModelConst));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_terrain, terrain, sizeof(TerrainSlot) * kMaxTerrainSlots);
 #if TRL_TABLE_MIRROR
     if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_model, &mc, sizeof(ModelConst));
 #endif
@@ -1675,7 +1707,7 @@ void launch_reset(const Buffers& B, const uint64_t* seeds, const int* env_ids, i
 
 }  // namespace TRL_IMPL_NS
 
-#if !defined(TRL_CG_VARIANT)
+#if !defined(TRL_CG_VARIANT) && !defined(TRL_TERRAIN_SLOTS_VARIANT)
 #include "trl_decide.cuh"
 #include "trl_decide2.cuh"
 #endif

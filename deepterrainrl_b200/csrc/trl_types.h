@@ -68,7 +68,12 @@ enum IField : int {
     I_SEG_N0, I_SEG_N1, I_SEG_FLIP, I_TERRAIN_RNG,   // minstd_rand0 state of the env's terrain generator
     I_TUPLE_FLAGS, I_RNG_CTR_LO, I_RNG_CTR_HI, I_STEPS_LO, I_STEPS_HI,
     I_STANCE,           // raptor: 0 = right leg is the stance leg, 1 = left
-    I_NUM_FIELDS
+    I_NUM_FIELDS,
+    // terrain slots (trl_load_terrain): planes past the fields the env-step kernel stages, read and written only where the ground is
+    // generated.  reset_env copies the assignment into the current slot before ResetGround
+    I_TERRAIN_SLOT = I_NUM_FIELDS,   // slot the env's present terrain was generated from
+    I_TERRAIN_SLOT_NEXT,             // slot assigned by the host (trl_set_env_terrain), used from the env's next reset on
+    I_NUM_PLANES
 };
 
 struct PhysParams {
@@ -143,6 +148,15 @@ struct ModelConst {
     uint64_t rng_seed;
 };
 
+// Terrain slots: slot 0 is the scene's own terrain (ModelConst::terrain_type / terrain_params), slots 1 .. kMaxTerrainSlots - 1 are
+// loaded from terrain files; every slot holds its parameter sets blended with the handle's blend.  The table sits in __constant__
+// memory beside the model and is uploaded with it.
+constexpr int kMaxTerrainSlots = 8;
+struct TerrainSlot {
+    int type;
+    double params[kTerrainParams];
+};
+
 // Exploration settings can change between updates (cScenarioExp::SetExpRate/Temp/BaseActionRate).
 struct ExpSettings {
     int enable;
@@ -183,7 +197,7 @@ struct PolicySlots {
 struct Buffers {
     int n;                 // number of envs
     double* d;             // [D_NUM_FIELDS][n]
-    int* i;                // [I_NUM_FIELDS][n]
+    int* i;                // [I_NUM_PLANES][n]
     float* terrain;        // [n][2][kTerrainCap]
     double* poli_state;    // [n][S]   policy state built at the last decision
     double* net_out;       // [n][kMaxNetOut]

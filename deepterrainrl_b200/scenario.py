@@ -46,7 +46,7 @@ VARIANTS = {
     "smem_xchg_decide_tile4": ["-DTRL_SMEM_XCHG=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
     "all": ["-DTRL_SMEM_XCHG=1", "-DTRL_REUSE_KIN=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
 }
-STEP_UNITS = ("trl_step.cu", "trl_step_cg.cu")      # the only translation units the variant flags reach
+STEP_UNITS = ("trl_step.cu", "trl_step_cg.cu", "trl_step_ts.cu", "trl_step_ts_cg.cu")      # the only translation units the variant flags reach
 
 
 def _variant():
@@ -70,7 +70,8 @@ def library_path():
 
 def build_library(force=False, verbose=False):
     """Compile csrc/*.cu for sm_90a into lib/libterrainrl_b200.so (nvcc cross-compiles without a GPU).
-    trl_step_cg.cu is the env-step translation unit again with -Xptxas -dlcm=cg (L1-bypassing loads, see trl_step.cu).
+    trl_step_cg.cu is the env-step translation unit again with -Xptxas -dlcm=cg (L1-bypassing loads, see trl_step.cu);
+    trl_step_ts.cu / trl_step_ts_cg.cu are both again with terrain slots.
     With TRL_VARIANT set, the two env-step units are compiled with the variant's flags and linked with the product's other
     objects into lib/variants/<name>/."""
     variant = _variant()
@@ -82,7 +83,8 @@ def build_library(force=False, verbose=False):
             os.environ["TRL_VARIANT"] = prev
     out = library_path()
     csrc = os.path.join(_PKG, "csrc")
-    units = [("trl_step.cu", []), ("trl_step_cg.cu", ["-Xptxas", "-dlcm=cg"]), ("trl_host.cu", []), ("trl_train.cu", []),
+    units = [("trl_step.cu", []), ("trl_step_cg.cu", ["-Xptxas", "-dlcm=cg"]), ("trl_step_ts.cu", []), ("trl_step_ts_cg.cu", ["-Xptxas", "-dlcm=cg"]),
+             ("trl_host.cu", []), ("trl_train.cu", []),
              ("trl_comm.cu", []), ("trl_probe.cu", []), ("trl_tc_policy.cu", []), ("ref_loader.cpp", [])]
     deps = [os.path.join(csrc, f) for f in os.listdir(csrc)]
     deps.append(os.path.join(_ROOT, "include", "terrainrl_b200.h"))
@@ -128,6 +130,7 @@ EXPORTS = [
     "trl_comm_broadcast_weights", "trl_comm_eval_stats", "trl_trainer_replica_spread", "trl_trainer_set_async",
     "trl_tc_split", "trl_tc_fc", "trl_tc_last_error", "trl_bench_last_span",
     "trl_load_policy", "trl_set_env_policy", "trl_eval_stats_slot",
+    "trl_load_terrain", "trl_set_env_terrain", "trl_env_terrain", "trl_eval_stats_cell",
 ]
 
 
@@ -238,6 +241,25 @@ class BatchedScenario:
     def EnvPolicy(self):
         """the slot of every env"""
         return getattr(self, "_env_slot", np.zeros(self.num_envs, np.int32)).copy()
+
+    def LoadTerrain(self, slot, path):
+        """a terrain file of the reference's format (as -terrain_file) into terrain slot 1..7; envs move to it with SetEnvTerrain"""
+        self._ck(self.L.trl_load_terrain(self.h, int(slot), os.fspath(path).encode()))
+
+    def SetEnvTerrain(self, slots, env_ids=None):
+        """env_ids[k] (default: env k) generates its ground from terrain slot slots[k] from its next episode reset on"""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        if ids is not None and ids.size != s.size:
+            raise ValueError("SetEnvTerrain: one slot per env id")
+        self._ck(self.L.trl_set_env_terrain(self.h, _p(ids), _p(s), int(s.size)))
+
+    def EnvTerrain(self):
+        """(current, assigned): per env, the terrain slot its present ground came from and the one it uses after its next reset"""
+        cur = np.zeros(self.num_envs, np.int32)
+        nxt = np.zeros(self.num_envs, np.int32)
+        self._ck(self.L.trl_env_terrain(self.h, _p(cur), _p(nxt), self.num_envs))
+        return cur, nxt
 
     def GetOutputOffsetScale(self):
         """cBaseControllerMACE::BuildNNOutputOffsetScale."""
@@ -389,14 +411,21 @@ class BatchedScenario:
     def GetNumEnvSteps(self):
         return self._stats()["steps"]
 
-    def GetEvalStats(self, slot=0):
-        """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot`"""
+    def GetEvalStats(self, slot=0, terrain=None):
+        """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot` (None: any) whose present ground comes from
+        terrain slot `terrain` (None: any)"""
         c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
-        self._ck(self.L.trl_eval_stats_slot(self.h, int(slot), C.byref(c), C.byref(e), C.byref(a), C.byref(s)))
+        if terrain is None and slot is not None:
+            rc = self.L.trl_eval_stats_slot(self.h, int(slot), C.byref(c), C.byref(e), C.byref(a), C.byref(s))
+        else:
+            rc = self.L.trl_eval_stats_cell(self.h, -1 if slot is None else int(slot), -1 if terrain is None else int(terrain),
+                                            C.byref(c), C.byref(e), C.byref(a), C.byref(s))
+        self._ck(rc)
         return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
 
-    def GetDistLog(self, slot=None):
-        """(distances, env ids) of the episodes logged so far; slot: only the entries of envs now on that policy slot"""
+    def GetDistLog(self, slot=None, terrain=None):
+        """(distances, env ids) of the episodes logged so far; slot / terrain: only the entries of envs now on that policy slot / whose
+        present ground comes from that terrain slot"""
         d = C.c_void_p(); e = C.c_void_p(); n = C.c_int(0)
         self._ck(self.L.trl_dist_log(self.h, C.byref(d), C.byref(e), C.byref(n)))
         if n.value == 0:
@@ -405,6 +434,9 @@ class BatchedScenario:
         env = np.ctypeslib.as_array(C.cast(e, C.POINTER(C.c_int32)), (n.value,)).copy()
         if slot is not None:
             keep = self.EnvPolicy()[env] == slot
+            dist, env = dist[keep], env[keep]
+        if terrain is not None:
+            keep = self.EnvTerrain()[0][env] == terrain
             dist, env = dist[keep], env[keep]
         return dist, env
 

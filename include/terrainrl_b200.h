@@ -177,6 +177,24 @@ int trl_get_output_offset_scale(trl_handle* h, double* offset, double* scale, in
 int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* scale_json_path);
 int trl_set_env_policy(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n);
 int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps);
+
+/* terrain slots: one handle (any mode, trainer or not) generates the ground of each env from one of up to 8 terrains.  Slot 0 is the
+ * scene's own terrain (the pack's, or -terrain_file); slots 1..7 start empty.  Every slot blends its parameter sets with the handle's
+ * blend (-terrain_blend, then trl_set_terrain_lerp, which re-blends every loaded slot).  Env i computes exactly what env i of a handle
+ * created with its slot's file as -terrain_file computes, with the same seeds.
+ *   trl_load_terrain     a terrain file of the reference's format ({"Type": ..., "Params": [...]}, read as -terrain_file is) into slot
+ *                        1..7; refused (handle unchanged) for slot 0 or >= 8, a null path, an unknown type or malformed JSON.
+ *   trl_set_env_terrain  env_ids[k] (NULL: env k) -> slots[k] for k < n; every env starts on slot 0.  Refused, with nothing changed,
+ *                        for an env id or slot out of range, n > num_envs or an empty slot.  Takes effect at the env's next episode
+ *                        reset (a fall inside trl_update, trl_reset, trl_seed_terrain): the ground already generated stays until then.
+ *   trl_env_terrain      per env (first n), the slot its present ground came from and the slot it will use after its next reset.
+ *   trl_eval_stats_cell  trl_eval_stats over the envs now on policy slot `policy_slot` and whose present ground comes from terrain slot
+ *                        `terrain_slot`; -1 = any slot.  trl_eval_stats_slot(h, p) is the cell (p, -1). */
+int trl_load_terrain(trl_handle* h, int slot, const char* terrain_json_path);
+int trl_set_env_terrain(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n);
+int trl_env_terrain(trl_handle* h, int32_t* current, int32_t* assigned, int n);
+int trl_eval_stats_cell(trl_handle* h, int policy_slot, int terrain_slot, int64_t* cycles, int64_t* episodes, double* avg_dist,
+                        int64_t* env_steps);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
