@@ -305,8 +305,10 @@ trl_fwd_conv_train_kernel(NetWeights W, FwdTrain f, double* __restrict__ act2) {
 // ------------------------------------------------------------------------------------------------ FC stage
 // the scalar decision of one env (cDogControllerMACE::UpdateAction, cBaseControllerMACE::DecideActionBoltzmann, BuildActorAction,
 // ApplyExpNoiseAction: sim/DogController.cpp:847-868, sim/BaseControllerMACE.cpp:254-318,339-396,437-518); Y = this decision's
-// unnormalised net output (unused when the scene has no net)
-__device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, const double* Y) {
+// unnormalised net output (unused when the scene has no net).  kSlots: the exploration noise is scaled by the deciding slot's own actor
+// output scale `noise_scale` (the net of a training slot sets it); otherwise by the scene's, c_model.out_scale_actor0
+template <bool kSlots = false>
+__device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, const double* Y, const double* noise_scale = nullptr) {
     const ModelConst& m = c_model;
     Lane L{nullptr, env, B.n, B.d, B.i};
     double params[kNumParams];
@@ -345,7 +347,7 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
             if (ex.enable) {
                 const double rn = rng.uniform();
                 if (rn < ex.rate) {              // ApplyExpNoiseAction
-                    for (int k = 0; k < fs; ++k) params[m.opt_idx[k]] += (ex.noise * rng.normal()) * (1.0 / m.out_scale_actor0[k]);
+                    for (int k = 0; k < fs; ++k) params[m.opt_idx[k]] += (ex.noise * rng.normal()) * (1.0 / (kSlots ? noise_scale[k] : m.out_scale_actor0[k]));
                     eflags |= 2;
                 }
                 if (a != a_max) eflags |= 1;
@@ -634,7 +636,10 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0,
             stamp();     // 11
         }
         // ---------------- the scalar decisions of this chunk, one lane each
-        if (!kTrain && rank == 0 && tid < rows) decide_one(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride);
+        if (!kTrain && rank == 0 && tid < rows) {
+            if (kSlots) decide_one<true>(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride, W.out_scale + n_frags);
+            else decide_one(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride);
+        }
         stamp();         // 12: decisions applied
         cluster.sync();      // Y / H / HH / the pipeline buffers are reused by the next chunk
         stamp();         // 13

@@ -55,6 +55,11 @@ struct trl_handle {
     std::vector<int> env_slot_host;
     trl::PolicySlots P{};                                    // device views (env_slot, weight table, sort scratch, chunk tables)
     trl::FcSlotMaps slot_maps{};
+    // training slots (trl_trainer_create_slot, exploration handles only): slot p >= 1 trains with slot_trainer[p], whose current net is
+    // slot_W[p]; slot 0's trainer stays `trainer`.  train_slots stays set once a slot trainer was created: the tuple block is then
+    // shared by slot, and its hand-over no longer clears it (trl_train_run_slots does, once every trainer has taken its rows)
+    bool train_slots = false;
+    trl_trainer* slot_trainer[trl::kMaxPolicySlots] = {};    // [0] unused
     // terrain slots (trl_load_terrain, any mode): slot 0 is mc.terrain_type / terrain_params, slots 1.. keep a terrain file's parameter
     // sets, blended at terrain_lerp into terrain[] (the __constant__ table, uploaded with the model).  Until a slot >= 1 is loaded
     // env_terrain_host is empty and every env is on slot 0 (the planes I_TERRAIN_SLOT / I_TERRAIN_SLOT_NEXT stay zero)
@@ -98,3 +103,6 @@ void trl_drop_graphs(trl_handle* h);
 extern "C" void trl_trainer_orphan(trl_trainer* t);              // trl_destroy with a trainer still attached (trl_train.cu)
 int trl_make_fc_maps(trl::FcMaps* out, const double* tip0_w, const double* act2, int rows);   // trl_host.cu
 int trl_reupload_model(trl_handle* h);                // after editing h->mc: refresh the __constant__ copies                  // captured graphs bake kernel arguments (weight pointers) in
+// policy slot `slot` >= 1 gets its own blobs holding the Caffe-HDF5 model + `_scale.txt` (both paths given) or a copy of slot 0's
+// current net, and the handle gets its slot machinery; refused, with nothing changed, for a model of another topology
+extern "C" int trl_stage_slot_model(trl_handle* h, int slot, const char* h5_path, const char* scale_path);

@@ -785,6 +785,8 @@ int trl_destroy(trl_handle* h) {
     if (!h) return 0;
     if (h->comm) trl_comm_destroy(h);
     if (h->trainer) trl_trainer_orphan(h->trainer);   // the trainer object outlives its scenario as an inert shell
+    for (int p = 1; p < kMaxPolicySlots; ++p)
+        if (h->slot_trainer[p]) trl_trainer_orphan(h->slot_trainer[p]);
     if (g_model_owner == h) g_model_owner = nullptr;
     if (h->stream) cudaStreamSynchronize(h->stream);
     destroy_graphs(h);
@@ -939,12 +941,20 @@ int trl_write_model(const char* path, const double* const* blobs, int n_char, in
     }
     return 0;
 }
+static int drain(trl_handle* h);
 // the policy the scenario currently evaluates (the attached trainer's net if there is one)
 int trl_output_model(trl_handle* h, const char* path, uint32_t mtime) {
     if (!h) return fail("trl_output_model: null handle");
+    return trl_output_model_slot(h, 0, path, mtime);
+}
+// the policy of slot `slot` (its trainer's net if it has one)
+int trl_output_model_slot(trl_handle* h, int slot, const char* path, uint32_t mtime) {
+    if (!h) return fail("trl_output_model_slot: null handle");
     if (!h->mc.has_net) return fail("trl_output_model: scene has no policy net");
-    CK(cudaStreamSynchronize(h->stream));
-    const NetWeights& W = h->W;
+    if (slot < 0 || slot >= kMaxPolicySlots) return fail("trl_output_model_slot: slot " + std::to_string(slot) + " out of range");
+    if (slot > 0 && h->slot_blobs[slot].empty()) return fail("trl_output_model_slot: slot " + std::to_string(slot) + " is empty");
+    if (drain(h)) return 1;
+    const NetWeights& W = slot == 0 ? h->W : h->slot_W[slot];
     const double* dev[30] = {W.conv0_w, W.conv0_b, W.conv1_w, W.conv1_b, W.conv2_w, W.conv2_b, W.tip0_w, W.tip0_b, W.ip0_w, W.ip0_b};
     for (int k = 0; k < 4; ++k) { dev[10 + 4 * k] = W.h0_w[k]; dev[11 + 4 * k] = W.h0_b[k]; dev[12 + 4 * k] = W.h1_w[k]; dev[13 + 4 * k] = W.h1_b[k]; }
     dev[26] = W.in_off; dev[27] = W.in_scale; dev[28] = W.out_off; dev[29] = W.out_scale;
@@ -1009,6 +1019,49 @@ static int drain(trl_handle* h) {
     return 0;
 }
 
+// the slot machinery, allocated with a handle's first slot >= 1: per-env slots (all 0), weight table, sort scratch and chunk tables
+static int ensure_policy_slots(trl_handle* h) {
+    if (h->P.W) return 0;
+    PolicySlots& P = h->P;
+    int* env_slot = nullptr;
+    NetWeights* table = nullptr;
+    const size_t n = (size_t)h->n;
+    P.chunk_cap = h->n / 32 + kMaxPolicySlots;
+    CK(dalloc(h, &env_slot, n));
+    CK(dalloc(h, &table, (size_t)kMaxPolicySlots));
+    CK(dalloc(h, &P.sort_tmp, (size_t)h->lag * n));
+    CK(dalloc(h, &P.chunks, (size_t)h->lag * (1 + 3 * P.chunk_cap)));
+    P.env_slot = env_slot; P.W = table;
+    h->env_slot_host.assign(n, 0);
+    return 0;
+}
+
+int trl_stage_slot_model(trl_handle* h, int slot, const char* h5_path, const char* scale_path) {
+    const int64_t vcounts[4] = {h->mc.n_in, h->mc.n_in, h->mc.n_out, h->mc.n_out};
+    if (h5_path && scale_path)
+        return read_model_files(h, "trl_trainer_create_slot", h5_path, scale_path, [&](const double* const* blobs, const int64_t* counts, std::vector<double>* vec) {
+            if (check_net_counts(h->mc, counts, vcounts)) return 1;
+            if (drain(h) || ensure_policy_slots(h)) return 1;
+            const double* vecs[4] = {vec[0].data(), vec[1].data(), vec[2].data(), vec[3].data()};
+            return upload_net(h, blobs, counts, vecs, vcounts, slot);
+        });
+    // a copy of the net slot 0 evaluates now (its trainer's, if it has one)
+    if (drain(h) || ensure_policy_slots(h)) return 1;
+    std::vector<double*>& dst = h->slot_blobs[slot];
+    if (dst.empty()) {
+        dst.assign(30, nullptr);
+        for (int i = 0; i < 30; ++i) CK(dalloc(h, &dst[i], (size_t)h->net_counts[i]));
+    }
+    const NetWeights& W = h->W;
+    const double* src[30] = {W.conv0_w, W.conv0_b, W.conv1_w, W.conv1_b, W.conv2_w, W.conv2_b, W.tip0_w, W.tip0_b, W.ip0_w, W.ip0_b};
+    for (int k = 0; k < 4; ++k) { src[10 + 4 * k] = W.h0_w[k]; src[11 + 4 * k] = W.h0_b[k]; src[12 + 4 * k] = W.h1_w[k]; src[13 + 4 * k] = W.h1_b[k]; }
+    src[26] = W.in_off; src[27] = W.in_scale; src[28] = W.out_off; src[29] = W.out_scale;
+    for (int i = 0; i < 30; ++i) CK(cudaMemcpy(dst[i], src[i], (size_t)h->net_counts[i] * 8, cudaMemcpyDeviceToDevice));
+    double** b = dst.data();
+    h->slot_W[slot] = net_weights(b, b[26], b[27], b[28], b[29]);
+    return 0;
+}
+
 static bool slot_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxPolicySlots && !h->slot_blobs[slot].empty()); }
 
 int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* scale_path) {
@@ -1024,19 +1077,7 @@ int trl_load_policy(trl_handle* h, int slot, const char* h5_path, const char* sc
         const int64_t vcounts[4] = {h->mc.n_in, h->mc.n_in, h->mc.n_out, h->mc.n_out};
         if (check_net_counts(h->mc, counts, vcounts)) return 1;
         if (drain(h)) return 1;
-        if (!h->P.W) {      // first slot of this handle: per-env slots (all 0), weight table, sort scratch and chunk tables
-            PolicySlots& P = h->P;
-            int* env_slot = nullptr;
-            NetWeights* table = nullptr;
-            const size_t n = (size_t)h->n;
-            P.chunk_cap = h->n / 32 + kMaxPolicySlots;
-            CK(dalloc(h, &env_slot, n));
-            CK(dalloc(h, &table, (size_t)kMaxPolicySlots));
-            CK(dalloc(h, &P.sort_tmp, (size_t)h->lag * n));
-            CK(dalloc(h, &P.chunks, (size_t)h->lag * (1 + 3 * P.chunk_cap)));
-            P.env_slot = env_slot; P.W = table;
-            h->env_slot_host.assign(n, 0);
-        }
+        if (ensure_policy_slots(h)) return 1;
         const double* vecs[4] = {vec[0].data(), vec[1].data(), vec[2].data(), vec[3].data()};
         if (upload_net(h, blobs, counts, vecs, vcounts, slot)) return 1;
         h->slots_active = true;
@@ -1059,9 +1100,20 @@ int trl_set_env_policy(trl_handle* h, const int32_t* env_ids, const int32_t* slo
     std::vector<int> next = h->env_slot_host;
     for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = slots[k];
     if (drain(h)) return 1;
+    std::vector<int32_t> moved;
+    if (h->train_slots) {
+        // every tuple belongs to the slot that chose its action: no move while the block holds tuples, and a moved env starts over
+        // (cScenarioExp::Reset zeroes its cycle count, so its unfinished cycle records no tuple)
+        int held = 0;
+        CK(cudaMemcpy(&held, h->B.tuple_count, 4, cudaMemcpyDeviceToHost));
+        if (held != 0)
+            return fail("trl_set_env_policy: the tuple block holds " + std::to_string(held) + " tuples of the present assignment (hand them over or trl_reset_tuples first)");
+        for (int e = 0; e < h->n; ++e)
+            if (next[e] != h->env_slot_host[e]) moved.push_back(e);
+    }
     CK(cudaMemcpy((void*)h->P.env_slot, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
     h->env_slot_host.swap(next);
-    return 0;
+    return moved.empty() ? 0 : trl_reset(h, moved.data(), (int)moved.size());
 }
 
 static bool terrain_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxTerrainSlots && h->terrain_loaded[slot]); }

@@ -342,6 +342,46 @@ __global__ void k_add_copy(Dev d, const double* rows, const uint32_t* src_flags)
     if (threadIdx.x == 0) d.flags[t] = (int)src_flags[i];
 }
 
+// ---- the slot-filtered hand-over of a handle with training slots (trl_train_run_slots): trainer p takes the rows whose env is on
+// policy slot p, in the order of its envs' ids, and leaves the rest of the block to the other trainers.  k_add_assign / k_add_copy
+// serve it unchanged: the slot's rows come first in d.order, every other row is invalid and takes no replay slot, so the replay memory
+// sees exactly the batches of 32 a single trainer fed only this slot's rows (in env order) sees.
+struct SlotRows { const int* env_ids; const int* env_slot; int slot; };
+__device__ __forceinline__ bool slot_row(const SlotRows& s, int i) { return s.env_slot[s.env_ids[i]] == s.slot; }
+__global__ void k_add_check_slot(Dev d, const double* rows, const int* count_ptr, SlotRows s) {
+    pdl_sync();
+    const int count = min(*count_ptr, (int)gridDim.x), i = blockIdx.x;
+    if (i >= count) return;
+    const double* r = rows + (size_t)i * d.Wd;
+    const bool mine = slot_row(s, i);
+    int bad = !mine;
+    if (mine)
+        for (int k = threadIdx.x; k < d.Wd; k += blockDim.x) bad |= !isfinite(r[k]);
+    bad = __syncthreads_or(bad);
+    if (threadIdx.x == 0) d.valid[i] = !bad;
+}
+// rank = #rows of the same slot with a smaller env id; the other rows are ranked after all of them (key bit 30)
+__global__ void k_add_order_slot(Dev d, const int* count_ptr, SlotRows s) {
+    pdl_sync();
+    const int count = min(*count_ptr, (int)gridDim.x), i = blockIdx.x;
+    if (i >= count) return;
+    const int key = s.env_ids[i] | (slot_row(s, i) ? 0 : 0x40000000);
+    int r = 0;
+    for (int j = threadIdx.x; j < count; j += blockDim.x) {
+        const int kj = s.env_ids[j] | (slot_row(s, j) ? 0 : 0x40000000);
+        r += (kj < key) || (kj == key && j < i);
+    }
+    __shared__ int red[32];
+    for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = r;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int tot = 0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+        d.order[tot] = i;
+    }
+}
+
 // ---- tuples from the all-gathered blocks of every rank (trl_comm.cu: {i32 count, i32 queued, i32 rank, i32 R, u32 flags[R],
 // i32 env[R], f32 rows[R][Wd]} per rank).  Arrival order = rank order, env order inside a rank: the same on every rank, so
 // replicated trainers stay bit-identical.  The validity bit (cNeuralNetTrainer::CheckTuple on the f64 values) was set by the
@@ -774,6 +814,9 @@ struct trl_trainer {
     double* snap = nullptr;            // [P + 2 S + 2 n_out]: theta, in_off, in_scale, out_off, out_scale as the decision kernels see them
     cudaStream_t work() const { return async ? async_stream : h->stream; }
     int64_t launches = 0;
+    int slot = 0;                      // policy slot whose net this trainer is (0: the handle's own, h->trainer)
+    cudaStream_t own_stream = nullptr; // trl_train_run_slots: hand-over + iterations of this trainer beside the other trainers'
+    cudaEvent_t ev_own = nullptr;
 };
 
 #define TCK(call)                                                                                       \
@@ -924,16 +967,31 @@ int enqueue_add(trl_trainer* t, const double* rows, const uint32_t* flags, const
     t->launches += 3;
     return 0;
 }
+// the hand-over of a handle with training slots: this trainer's slot's rows of the scene's block; the block stays for the others
+void enqueue_add_slot(trl_trainer* t, cudaStream_t st) {
+    const Dev& d = t->d;
+    const trl_handle* h = t->h;
+    const int max_count = h->B.tuple_cap;
+    const SlotRows s{h->B.tuple_env, h->P.env_slot, t->slot};
+    launch_pdl(k_add_check_slot, dim3(max_count), dim3(128), 0, st, d, (const double*)h->B.tuples, (const int*)h->B.tuple_count, s);
+    launch_pdl(k_add_order_slot, dim3(max_count), dim3(128), 0, st, d, (const int*)h->B.tuple_count, s);
+    launch_pdl(k_add_assign, dim3(1), dim3(32), 0, st, d, (const uint32_t*)h->B.tuple_flags, (const int*)h->B.tuple_count, 0, max_count, (int*)nullptr, 1);
+    launch_pdl(k_add_copy, dim3(max_count), dim3(128), 0, st, d, (const double*)h->B.tuples, (const uint32_t*)h->B.tuple_flags);
+    t->launches += 4;
+}
+
+void trainer_free(trl_trainer* t) {
+    for (void* q : t->allocs) cudaFree(q);
+    delete t;
+}
 }  // namespace
 
 extern "C" {
 
 // p[10]: replay_cap, num_init_samples, num_steps_per_iter, freeze_target_iters, init_input_offset_scale, discount, base_lr,
 //        momentum, weight_decay, seed   (cTrainerInterface::tParams + the solver prototxt)
-trl_trainer* trl_trainer_create(trl_handle* h, const double* p) {
-    if (!h || !h->mc.has_net) { trl_fail("trl_trainer_create: the scene has no policy net"); return nullptr; }
-    if (h->trainer) { trl_fail("trl_trainer_create: a trainer is already attached"); return nullptr; }
-    if (h->slots_active) { trl_fail("trl_trainer_create: the handle evaluates several policy slots (trl_load_policy); a trainer needs a single-policy handle"); return nullptr; }
+// the trainer's dimensions and device buffers; the handle is not touched (nullptr, with the reason recorded, on failure)
+static trl_trainer* trainer_new(trl_handle* h, const double* p) {
     auto* t = new trl_trainer();
     t->h = h;
     Dev& d = t->d;
@@ -994,32 +1052,77 @@ trl_trainer* trl_trainer_create(trl_handle* h, const double* p) {
     if (ok) {
         A(cudaMemset(d.pos_critic, 0xff, (size_t)d.cap * 4));
         A(cudaMemset(d.pos_actor, 0xff, (size_t)d.cap * 4));
-        cudaStreamSynchronize(h->stream);
-        // LoadModel: start from the engine's current policy (weights + offset / scale); the target net is a copy
-        for (int b = 0; b < 26 && ok; ++b) A(cudaMemcpy(d.theta + d.off[b], h->net_blobs[b], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice));
-        A(cudaMemcpy(d.target, d.theta, (size_t)d.P * 8, cudaMemcpyDeviceToDevice));
-        double* dst[8] = {d.in_off, d.in_scale, d.out_off, d.out_scale, d.t_in_off, d.t_in_scale, d.t_out_off, d.t_out_scale};
-        for (int k = 0; k < 8 && ok; ++k) A(cudaMemcpy(dst[k], h->net_blobs[26 + (k & 3)], (size_t)h->net_counts[26 + (k & 3)] * 8, cudaMemcpyDeviceToDevice));
     }
     if (!ok) {
-        for (void* q : t->allocs) cudaFree(q);
-        delete t;
+        trainer_free(t);
         return nullptr;
     }
+    return t;
+}
+// LoadModel: start from the 26 blobs + 4 offset / scale vectors of `src` (the engine's copy of the slot's policy); the target net is a
+// copy.  Then the descriptors of the trainer's own forward passes
+static int trainer_start(trl_trainer* t, const std::vector<double*>& src) {
+    trl_handle* h = t->h;
+    Dev& d = t->d;
+    bool ok = true;
+    auto A = [&](cudaError_t e) { if (e != cudaSuccess) { if (ok) trl_fail(std::string("trainer load: ") + cudaGetErrorString(e)); ok = false; } };
+    cudaStreamSynchronize(h->stream);
+    for (int b = 0; b < 26 && ok; ++b) A(cudaMemcpy(d.theta + d.off[b], src[b], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice));
+    A(cudaMemcpy(d.target, d.theta, (size_t)d.P * 8, cudaMemcpyDeviceToDevice));
+    double* dst[8] = {d.in_off, d.in_scale, d.out_off, d.out_scale, d.t_in_off, d.t_in_scale, d.t_out_off, d.t_out_scale};
+    for (int k = 0; k < 8 && ok; ++k) A(cudaMemcpy(dst[k], src[26 + (k & 3)], (size_t)h->net_counts[26 + (k & 3)] * 8, cudaMemcpyDeviceToDevice));
+    if (!ok) return 1;
     const double* blobs[2][26];            // the blobs of the current net (in theta) and of the target net (in target)
     for (int b = 0; b < 26; ++b) { blobs[0][b] = d.theta + d.off[b]; blobs[1][b] = d.target + d.off[b]; }
     for (int k = 0; k < 2; ++k) {
         t->nw[k] = net_weights(blobs[k], nullptr, nullptr, nullptr, nullptr);     // the minibatch arrives normalised; outputs stay normalised
-        if (trl_make_fc_maps(&t->fmaps[k], t->nw[k].tip0_w, d.a2, 3 * kB)) {
-            for (void* q : t->allocs) cudaFree(q);
-            delete t;
-            return nullptr;
-        }
+        if (trl_make_fc_maps(&t->fmaps[k], t->nw[k].tip0_w, d.a2, 3 * kB)) return 1;
     }
-    // cNeuralNetLearner::SyncNet as a binding: the decision kernel reads the trainer's weights from now on
-    h->W = net_weights(blobs[0], d.in_off, d.in_scale, d.out_off, d.out_scale);
+    return 0;
+}
+
+trl_trainer* trl_trainer_create(trl_handle* h, const double* p) { return trl_trainer_create_slot(h, 0, p, nullptr, nullptr); }
+
+// A trainer for policy slot `slot`: slot 0 is the handle's own policy (trl_trainer_create); slots 1..7 are training slots of an
+// exploration handle, whose envs (trl_set_env_policy) explore with the slot trainer's net and feed it their tuples
+trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* p, const char* h5_path, const char* scale_path) {
+    auto refuse = [](const std::string& why) -> trl_trainer* { trl_fail(why); return nullptr; };
+    if (!h || !h->mc.has_net) return refuse("trl_trainer_create: the scene has no policy net");
+    if (slot < 0 || slot >= kMaxPolicySlots) return refuse("trl_trainer_create_slot: slot " + std::to_string(slot) + " out of range (0.." + std::to_string(kMaxPolicySlots - 1) + ")");
+    if (slot == 0) {
+        if (h->trainer) return refuse("trl_trainer_create: a trainer is already attached");
+        if (h->slots_active && !h->train_slots)
+            return refuse("trl_trainer_create: the handle evaluates several policy slots (trl_load_policy); a trainer needs a single-policy handle");
+    } else {
+        if (h->mode != TRL_MODE_EXPLORE) return refuse("trl_trainer_create_slot: training slots are for exploration handles (TRL_MODE_EXPLORE)");
+        if (h->slot_trainer[slot]) return refuse("trl_trainer_create_slot: slot " + std::to_string(slot) + " already has a trainer");
+        if (!h->decide_v2) return refuse("trl_trainer_create_slot: the TRL_DECIDE_V1 decision kernel has no policy slots");
+        if (h->comm) return refuse("trl_trainer_create_slot: training slots do not exchange tuples between GPUs (the handle has a communicator)");
+    }
+    trl_trainer* t = trainer_new(h, p);
+    if (!t) return nullptr;
+    t->slot = slot;
+    const bool files = h5_path && scale_path;
+    const int rc = slot == 0 ? (files ? trl_load_model(h, h5_path, scale_path) : 0) : trl_stage_slot_model(h, slot, h5_path, scale_path);
+    if (rc || trainer_start(t, slot == 0 ? h->net_blobs : h->slot_blobs[slot])) {
+        trainer_free(t);
+        return nullptr;
+    }
+    // cNeuralNetLearner::SyncNet as a binding: the decision kernels read the trainer's weights from now on (a slot's through the slot
+    // table and its terr_ip0 descriptor, rewritten by ensure_slot_tables before the next decision)
+    const Dev& d = t->d;
+    const double* blobs[26];
+    for (int b = 0; b < 26; ++b) blobs[b] = d.theta + d.off[b];
+    if (slot == 0) {
+        h->W = net_weights(blobs, d.in_off, d.in_scale, d.out_off, d.out_scale);
+        h->trainer = t;
+    } else {
+        h->slot_W[slot] = net_weights(blobs, d.in_off, d.in_scale, d.out_off, d.out_scale);
+        h->slot_trainer[slot] = t;
+        h->slots_active = h->train_slots = true;
+        h->slot_dirty = true;
+    }
     trl_drop_graphs(h);
-    h->trainer = t;
     return t;
 }
 
@@ -1033,16 +1136,18 @@ void trl_trainer_orphan(trl_trainer* t) {
         cudaStreamSynchronize(t->async_stream); cudaStreamDestroy(t->async_stream); cudaEventDestroy(t->ev_snap); cudaEventDestroy(t->ev_trained);
         t->async_stream = nullptr; t->async = false;
     }
+    if (t->own_stream) { cudaStreamSynchronize(t->own_stream); cudaStreamDestroy(t->own_stream); cudaEventDestroy(t->ev_own); t->own_stream = nullptr; }
     if (t->train_graph) { cudaGraphExecDestroy(t->train_graph); t->train_graph = nullptr; }
     for (void* q : t->allocs) cudaFree(q);
     t->allocs.clear();
-    t->h->trainer = nullptr;
+    (t->slot == 0 ? t->h->trainer : t->h->slot_trainer[t->slot]) = nullptr;
     t->h = nullptr;
 }
 #define TRL_TRAINER_LIVE(t) do { if (!(t) || !(t)->h) return trl_fail("trainer: the scenario it was attached to has been destroyed"); } while (0)
 static cudaError_t trainer_sync(trl_trainer* t) {
     cudaError_t e = cudaStreamSynchronize(t->h->stream);
     if (e == cudaSuccess && t->async_stream) e = cudaStreamSynchronize(t->async_stream);
+    if (e == cudaSuccess && t->own_stream) e = cudaStreamSynchronize(t->own_stream);
     return e;
 }
 
@@ -1051,14 +1156,28 @@ int trl_trainer_destroy(trl_trainer* t) {
     trl_handle* h = t->h;
     if (!h) { delete t; return 0; }
     cudaStreamSynchronize(h->stream);
-    // hand the weights back to the engine's own buffers so the scenario stays usable
-    for (int b = 0; b < 26; ++b) cudaMemcpy(h->net_blobs[b], t->d.theta + t->d.off[b], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice);
-    cudaMemcpy(h->net_blobs[26], t->d.in_off, (size_t)h->net_counts[26] * 8, cudaMemcpyDeviceToDevice);
-    cudaMemcpy(h->net_blobs[27], t->d.in_scale, (size_t)h->net_counts[27] * 8, cudaMemcpyDeviceToDevice);
-    double** b = h->net_blobs.data();
-    h->W = net_weights(b, b[26], b[27], b[28], b[29]);
+    if (t->own_stream) { cudaStreamSynchronize(t->own_stream); cudaStreamDestroy(t->own_stream); cudaEventDestroy(t->ev_own); }
+    if (t->slot == 0) {
+        // hand the weights back to the engine's own buffers so the scenario stays usable
+        for (int b = 0; b < 26; ++b) cudaMemcpy(h->net_blobs[b], t->d.theta + t->d.off[b], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice);
+        cudaMemcpy(h->net_blobs[26], t->d.in_off, (size_t)h->net_counts[26] * 8, cudaMemcpyDeviceToDevice);
+        cudaMemcpy(h->net_blobs[27], t->d.in_scale, (size_t)h->net_counts[27] * 8, cudaMemcpyDeviceToDevice);
+        double** b = h->net_blobs.data();
+        h->W = net_weights(b, b[26], b[27], b[28], b[29]);
+        h->trainer = nullptr;
+    } else {
+        // into the slot's own blobs, offset / scale vectors included (the slot's exploration noise is scaled by its output scale): the
+        // slot stays loaded with the trained net
+        std::vector<double*>& sb = h->slot_blobs[t->slot];
+        const double* vec[4] = {t->d.in_off, t->d.in_scale, t->d.out_off, t->d.out_scale};
+        for (int b = 0; b < 30; ++b)
+            cudaMemcpy(sb[b], b < 26 ? t->d.theta + t->d.off[b] : vec[b - 26], (size_t)h->net_counts[b] * 8, cudaMemcpyDeviceToDevice);
+        double** b = sb.data();
+        h->slot_W[t->slot] = net_weights(b, b[26], b[27], b[28], b[29]);
+        h->slot_dirty = true;
+        h->slot_trainer[t->slot] = nullptr;
+    }
     trl_drop_graphs(h);
-    h->trainer = nullptr;
     if (t->train_graph) cudaGraphExecDestroy(t->train_graph);
     if (t->async_stream) { cudaStreamSynchronize(t->async_stream); cudaStreamDestroy(t->async_stream); cudaEventDestroy(t->ev_snap); cudaEventDestroy(t->ev_trained); }
     for (void* q : t->allocs) cudaFree(q);
@@ -1070,7 +1189,8 @@ int trl_trainer_destroy(trl_trainer* t) {
 int trl_trainer_add_from_scene(trl_trainer* t) {
     TRL_TRAINER_LIVE(t);
     trl_handle* h = t->h;
-    enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, h->B.tuple_count, h->stream, h->B.tuple_env);
+    if (h->train_slots) enqueue_add_slot(t, h->stream);      // this slot's rows; the block stays for the other trainers
+    else enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, h->B.tuple_count, h->stream, h->B.tuple_env);
     TCK(cudaGetLastError());
     return 0;
 }
@@ -1146,27 +1266,30 @@ int trl_trainer_replica_spread(trl_trainer* t, double* max_abs_diff) {
     return trl_comm_replica_spread(t->h, t->d.theta, (size_t)t->d.P, max_abs_diff);
 }
 
-// `iters` x cNeuralNetTrainer::Train() on the engine's stream (ordered after the update that produced the tuples and before
-// the next one, which then evaluates the updated weights)
-int trl_trainer_train(trl_trainer* t, int iters) {
-    TRL_TRAINER_LIVE(t);
-    trl_handle* h = t->h;
+// `iters` replays of the captured training iteration on stream `st`
+static int train_on(trl_trainer* t, int iters, cudaStream_t st) {
     if (!t->train_graph) {
         cudaGraph_t graph;
         const int64_t before = t->launches;
-        TCK(cudaStreamBeginCapture(t->work(), cudaStreamCaptureModeThreadLocal));
-        enqueue_train(t, t->work());
-        TCK(cudaStreamEndCapture(t->work(), &graph));
+        TCK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+        enqueue_train(t, st);
+        TCK(cudaStreamEndCapture(st, &graph));
         TCK(cudaGraphInstantiate(&t->train_graph, graph, 0));
         cudaGraphDestroy(graph);
         t->graph_launches = t->launches - before;      // capturing ran no kernel; each replay runs the kernels it recorded
         t->launches = before;
     }
     for (int i = 0; i < iters; ++i) {
-        TCK(cudaGraphLaunch(t->train_graph, t->work()));
+        TCK(cudaGraphLaunch(t->train_graph, st));
         t->launches += t->graph_launches;
     }
     return 0;
+}
+// `iters` x cNeuralNetTrainer::Train() on the engine's stream (ordered after the update that produced the tuples and before
+// the next one, which then evaluates the updated weights)
+int trl_trainer_train(trl_trainer* t, int iters) {
+    TRL_TRAINER_LIVE(t);
+    return train_on(t, iters, t->work());
 }
 
 // Training from scratch: the net the reference builds when no -policy_model is given.
@@ -1211,6 +1334,7 @@ int trl_trainer_init_fresh(trl_trainer* t, uint64_t seed) {
         TCK(cudaMemcpy(oo[k], out_off.data(), (size_t)d.n_out * 8, cudaMemcpyHostToDevice));
         TCK(cudaMemcpy(os[k], out_scale.data(), (size_t)d.n_out * 8, cudaMemcpyHostToDevice));
     }
+    if (t->slot != 0) return 0;      // a training slot's exploration noise is scaled by the slot's own out_scale, just written
     for (int k = 0; k < fs; ++k) m.out_scale_actor0[k] = out_scale[nf + k];       // exploration noise scale of the decision kernel
     return trl_reupload_model(h);
 }
@@ -1230,6 +1354,7 @@ int trl_trainer_set_async(trl_trainer* t, int enable) {
     TRL_TRAINER_LIVE(t);
     trl_handle* h = t->h;
     if ((enable != 0) == t->async) return 0;
+    if (h->train_slots) return trl_fail("trl_trainer_set_async: the handle has training slots (their trainers run in lock-step: trl_train_run_slots)");
     TCK(trainer_sync(t));
     const Dev& d = t->d;
     if (t->train_graph) { cudaGraphExecDestroy(t->train_graph); t->train_graph = nullptr; }      // it was captured on the other stream
@@ -1342,6 +1467,7 @@ static int train_run_impl(trl_trainer* t, const double* sp, int num_updates, int
 }
 int trl_train_run(trl_trainer* t, const double* sp, int num_updates, int iters_per_update, int tuple_buffer_size, double time_step) {
     TRL_TRAINER_LIVE(t);
+    if (t->h->train_slots) return trl_fail("trl_train_run: the handle has training slots, whose trainers share its tuple block (trl_train_run_slots)");
     return train_run_impl(t, sp, num_updates, iters_per_update, tuple_buffer_size, time_step, 0, nullptr);
 }
 // the same loop, device-timed: CUDA events on the scenario's stream around `num_updates` iterations of {update, tuple exchange,
@@ -1351,6 +1477,7 @@ int trl_train_run_timed(trl_trainer* t, const double* sp, int num_updates, int i
     TRL_TRAINER_LIVE(t);
     if (iters_per_update <= 0) return trl_fail("trl_train_run_timed: iters_per_update must be positive (no read-backs inside a timed region)");
     trl_handle* h = t->h;
+    if (h->train_slots) return trl_fail("trl_train_run_timed: the handle has training slots, whose trainers share its tuple block (trl_train_run_slots)");
     const size_t flush_bytes = (size_t)256 << 20;
     if (flush_l2 && !h->flush_buf) { TCK(cudaMalloc(&h->flush_buf, flush_bytes)); h->allocs.push_back(h->flush_buf); }
     cudaEvent_t e0, e1;
@@ -1368,6 +1495,60 @@ int trl_train_run_timed(trl_trainer* t, const double* sp, int num_updates, int i
         if (ms) *ms = f;
     }
     cudaEventDestroy(e0); cudaEventDestroy(e1);
+    return rc;
+}
+
+// The trl_train_run loop for k trainers of one handle (slot 0's and / or training slots'), in lock-step: every update applies ONE
+// exploration setting and curriculum blend, those of the schedule at the iterations each trainer has done (the same for all,
+// iters_per_update each per update, counted from 0 in every call).  Per update: the update, then one branch per trainer on its own
+// stream -- its hand-over (its slot's rows of the block, in env order) and iters_per_update replays of its training iteration --,
+// the join, and the block's cursor back to zero.  Each trainer computes what a single-trainer handle fed only its slot's rows computes.
+int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp, int num_updates, int iters_per_update, double time_step) {
+    if (!ts || k < 1) return trl_fail("trl_train_run_slots: need at least one trainer");
+    for (int i = 0; i < k; ++i) {
+        TRL_TRAINER_LIVE(ts[i]);
+        if (ts[i]->h != ts[0]->h) return trl_fail("trl_train_run_slots: the trainers belong to different handles");
+        for (int j = 0; j < i; ++j)
+            if (ts[j] == ts[i]) return trl_fail("trl_train_run_slots: trainer " + std::to_string(i) + " is listed twice");
+        if (ts[i]->async) return trl_fail("trl_train_run_slots: asynchronous trainers are not run in lock-step");
+    }
+    if (iters_per_update <= 0) return trl_fail("trl_train_run_slots: iters_per_update must be positive (the trainers advance in lock-step)");
+    trl_handle* h = ts[0]->h;
+    if (h->comm) return trl_fail("trl_train_run_slots: the handle has a communicator (multi-GPU training runs through trl_train_run)");
+    for (int i = 0; i < k; ++i) {
+        trl_trainer* t = ts[i];
+        if (!t->own_stream) {
+            TCK(cudaStreamCreateWithFlags(&t->own_stream, cudaStreamNonBlocking));
+            TCK(cudaEventCreateWithFlags(&t->ev_own, cudaEventDisableTiming));
+        }
+    }
+    cudaEvent_t fork;
+    TCK(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
+    int rc = 0;
+    long long iters = 0;
+    double last_phase = -1.0;
+    for (int u = 0; u < num_updates && rc == 0; ++u) {
+        double s[4];
+        trl_train_schedule(sp, (int)std::min<long long>(iters, 2000000000LL), s);
+        if (trl_set_explore(h, 1, s[0], s[1], s[2])) { rc = 1; break; }
+        if (s[3] != last_phase) { if (trl_set_terrain_lerp(h, s[3])) { rc = 1; break; } last_phase = s[3]; }
+        if (trl_update(h, time_step)) { rc = 1; break; }
+        cudaEventRecord(fork, h->stream);
+        for (int i = 0; i < k && rc == 0; ++i) {
+            trl_trainer* t = ts[i];
+            cudaStreamWaitEvent(t->own_stream, fork, 0);
+            if (h->train_slots) enqueue_add_slot(t, t->own_stream);
+            else enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, nullptr, t->own_stream, h->B.tuple_env);
+            rc = train_on(t, iters_per_update, t->own_stream);
+            cudaEventRecord(t->ev_own, t->own_stream);
+        }
+        for (int i = 0; i < k; ++i) cudaStreamWaitEvent(h->stream, ts[i]->ev_own, 0);
+        cudaMemsetAsync(h->B.tuple_count, 0, 4, h->stream);      // cScenarioExp::ResetTupleBuffer, once every trainer has taken its rows
+        iters += iters_per_update;
+        const cudaError_t e = cudaGetLastError();
+        if (rc == 0 && e != cudaSuccess) rc = trl_fail(std::string("trl_train_run_slots: ") + cudaGetErrorString(e));
+    }
+    cudaEventDestroy(fork);
     return rc;
 }
 

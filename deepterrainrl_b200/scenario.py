@@ -131,6 +131,7 @@ EXPORTS = [
     "trl_tc_split", "trl_tc_fc", "trl_tc_last_error", "trl_bench_last_span",
     "trl_load_policy", "trl_set_env_policy", "trl_eval_stats_slot",
     "trl_load_terrain", "trl_set_env_terrain", "trl_env_terrain", "trl_eval_stats_cell",
+    "trl_trainer_create_slot", "trl_train_run_slots", "trl_output_model_slot",
 ]
 
 
@@ -213,9 +214,13 @@ class BatchedScenario:
         ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32)
         self._ck(self.L.trl_reset(self.h, _p(ids), 0 if ids is None else ids.size))
 
-    def OutputModel(self, path, mtime=0):
-        """cNeuralNet::OutputModel of the policy the scenario evaluates: Caffe-layout HDF5 + `<stem>_scale.txt`, written natively."""
-        self._ck(self.L.trl_output_model(self.h, path.encode(), C.c_uint32(mtime)))
+    def OutputModel(self, path, mtime=0, slot=0):
+        """cNeuralNet::OutputModel of the policy the scenario evaluates (of policy slot `slot`: its trainer's net if it has one):
+        Caffe-layout HDF5 + `<stem>_scale.txt`, written natively."""
+        if slot == 0:
+            self._ck(self.L.trl_output_model(self.h, path.encode(), C.c_uint32(mtime)))
+        else:
+            self._ck(self.L.trl_output_model_slot(self.h, int(slot), path.encode(), C.c_uint32(mtime)))
 
     def LoadModel(self, h5_path, scale_path=None):
         """cNeuralNet::LoadModel + LoadScale from the reference's file formats."""

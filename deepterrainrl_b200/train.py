@@ -129,3 +129,20 @@ class ScenarioTrainMACE:
         import time
         os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
         self.exp.OutputModel(path, mtime=int(time.time()))            # native writer behind the C ABI (csrc/model_io.h)
+
+
+def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step=1.0 / 30.0):
+    """cScenarioTrain::Run for several trainers of one exploration scenario (trl_train_run_slots): `num_updates` updates of the
+    whole batch, each followed by every trainer's hand-over of its slot's tuples and `iters_per_update` iterations, the trainers side by
+    side on their own streams.  The exploration settings and curriculum blend follow `schedule` at the iterations each trainer has done
+    in this call (the same for all)."""
+    trainers = list(trainers)
+    if not trainers:
+        raise ValueError("train_run_slots: no trainer")
+    L = trainers[0].L
+    arr = (C.c_void_p * len(trainers))(*[t.h.value if t.h is not None else None for t in trainers])
+    sp = np.array([schedule.p[k] for k in TrainSchedule.KEYS], float)
+    rc = L.trl_train_run_slots(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), int(iters_per_update),
+                               C.c_double(time_step))
+    if rc != 0:
+        raise RuntimeError(L.trl_last_error().decode())

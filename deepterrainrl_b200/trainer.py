@@ -2,6 +2,7 @@
 scenario it was created from: tuples move device to device, and the scenario's decision kernel evaluates the trainer's weights
 in place (learning/NeuralNetLearner.cpp:33-45,83-87)."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -22,11 +23,14 @@ class MACETrainer:
     DEFAULTS = dict(replay_mem_size=500000, num_init_samples=50000, num_steps_per_iter=1, freeze_target_iters=500,
                     init_input_offset_scale=1, discount=0.9, base_lr=1e-3, momentum=0.9, weight_decay=5e-4, seed=1)
 
-    def __init__(self, scenario, **kw):
+    def __init__(self, scenario, slot=0, model=None, **kw):
+        """slot: the policy slot this trainer trains (0: the scenario's own policy; 1..7: a training slot of an exploration
+        scenario, whose envs are moved to it with SetEnvPolicy).  model: (h5_path, scale_path) of the starting net; None = the net
+        slot 0 evaluates now."""
         self.L = load_library()
         L = self.L
-        L.trl_trainer_create.restype = C.c_void_p
-        L.trl_trainer_create.argtypes = [C.c_void_p, C.c_void_p]
+        L.trl_trainer_create_slot.restype = C.c_void_p
+        L.trl_trainer_create_slot.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_char_p, C.c_char_p]
         L.trl_trainer_launches.restype = C.c_int64
         for name in ("trl_trainer_destroy", "trl_trainer_add_from_scene", "trl_trainer_add_tuples", "trl_trainer_train",
                      "trl_trainer_add_device", "trl_trainer_counters", "trl_trainer_get", "trl_trainer_set_theta", "trl_trainer_list"):
@@ -37,7 +41,9 @@ class MACETrainer:
         arr = np.array([p[k] for k in ("replay_mem_size", "num_init_samples", "num_steps_per_iter", "freeze_target_iters",
                                        "init_input_offset_scale", "discount", "base_lr", "momentum", "weight_decay", "seed")], float)
         self.scenario = scenario
-        h = L.trl_trainer_create(scenario.h, _p(arr))
+        self.slot = int(slot)
+        h5, scale = (None, None) if model is None else (os.fspath(model[0]).encode(), os.fspath(model[1]).encode())
+        h = L.trl_trainer_create_slot(scenario.h, self.slot, _p(arr), h5, scale)
         if not h:
             raise RuntimeError(L.trl_last_error().decode())
         self.h = C.c_void_p(h)

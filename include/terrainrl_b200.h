@@ -159,6 +159,8 @@ int trl_debug_step_phases(trl_handle* h, unsigned long long* out, int n, int res
  *   trl_get_output_offset_scale   cBaseControllerMACE::BuildNNOutputOffsetScale (sim/BaseControllerMACE.cpp:75-113) */
 int trl_load_model(trl_handle* h, const char* h5_path, const char* scale_json_path);
 int trl_output_model(trl_handle* h, const char* path, uint32_t mtime);
+/* trl_output_model for the net policy slot `slot` evaluates (its trainer's, if it has one); slot 0 is trl_output_model */
+int trl_output_model_slot(trl_handle* h, int slot, const char* path, uint32_t mtime);
 int trl_write_model(const char* path, const double* const* blobs26, int n_char, int n_frags, int frag_size, const double* in_off,
                     const double* in_scale, const double* out_off, const double* out_scale, uint32_t mtime);
 int trl_get_output_offset_scale(trl_handle* h, double* offset, double* scale, int n_out);
@@ -169,7 +171,7 @@ int trl_get_output_offset_scale(trl_handle* h, double* offset, double* scale, in
  * single-policy handles would, env for env.
  *   trl_load_policy      Caffe-HDF5 model + `_scale.txt` into slot 1..7; refused (handle unchanged) for another topology, an
  *                        exploration handle, a handle with a trainer, and the TRL_DECIDE_V1 build.  trl_trainer_create refuses a
- *                        handle with a loaded slot >= 1.
+ *                        handle with a loaded slot >= 1.  (Slots that carry trainers: trl_trainer_create_slot below.)
  *   trl_set_env_policy   env_ids[k] (NULL: env k) -> slots[k] for k < n; every env starts on slot 0.  Refused, with nothing changed,
  *                        for an env id or slot out of range or an empty slot.  Takes effect at the env's next decision, no reset.
  *   trl_eval_stats_slot  trl_eval_stats over the envs now on `slot`.  trl_get_net_out / trl_get_layer_state / trl_debug_decide follow
@@ -235,6 +237,25 @@ int trl_trainer_get(trl_trainer* t, int what, double* out);
 int trl_trainer_set_theta(trl_trainer* t, const double* theta);
 int trl_trainer_list(trl_trainer* t, int which, int32_t* out, int cap, int* len);
 int trl_trainer_rows(trl_trainer* t, const int32_t* slots, int n, float* rows, int32_t* flags);
+
+/* training slots: one exploration handle (TRL_MODE_EXPLORE) trains up to 8 policies side by side, one trainer per policy slot, each
+ * env exploring with the net of its slot (trl_set_env_policy) and feeding that slot's trainer.  Env i on slot p computes exactly what
+ * env i computes in a single-trainer handle of the same pack, seeds and size whose trainer is fed only the tuples of slot p's envs,
+ * and trainer p ends with that trainer's weights, buffers and counters.
+ *   trl_trainer_create_slot  a trainer for slot 0 (the handle's own policy; trl_trainer_create(h, p) is the call with slot 0 and no
+ *                        paths) or a training slot 1..7.  The starting net is the Caffe-HDF5 model + `_scale.txt` if both paths are
+ *                        given, else a copy of the net slot 0 evaluates now.  Refused, with the handle unchanged, for a slot out of
+ *                        range or with a trainer, a slot >= 1 on an evaluation handle, in the TRL_DECIDE_V1 build or on a handle
+ *                        with a communicator, slot 0 on a handle with trl_load_policy slots, and a model of another topology.
+ *                        trl_trainer_destroy of a slot trainer leaves its trained net in the slot.
+ *   trl_train_run_slots  the trl_train_run loop for k trainers of one handle in lock-step (iters_per_update > 0 each per update,
+ *                        one exploration setting and curriculum blend per update, annealed from 0 in every call).  Refused for
+ *                        trainers of different handles, a trainer listed twice, k < 1 and iters_per_update <= 0.
+ * Once a handle has a training slot: trl_trainer_add_from_scene hands a trainer only its slot's tuples and leaves the block to the
+ * others (trl_reset_tuples clears it); trl_set_env_policy is refused while the block holds tuples and resets the envs it moves, so
+ * every tuple belongs to the slot that chose its action; trl_train_run / trl_train_run_timed / trl_trainer_set_async are refused. */
+trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* params10, const char* h5_path, const char* scale_json_path);
+int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp9, int num_updates, int iters_per_update, double time_step);
 
 /* number of tuples the engine could not record because the tuple block was full (cScenarioExp's ring overwrites, scenarios/
  * ScenarioExp.cpp:296-301; a batch block refuses instead and counts).  trl_num_tuples / trl_get_tuples* return
