@@ -29,6 +29,7 @@
 #include <algorithm>
 #include <cmath>
 
+#include "trl_rcp.cuh"
 #include "trl_terrain.cuh"
 #include "trl_types.h"
 
@@ -661,10 +662,8 @@ __device__ __forceinline__ void chain_inward(double* xs, const ChainC& ch, int l
 #pragma unroll
     for (int k = 0; k < NV; ++k) a[k] = 0.0;
     for (int lev = 0; lev < m.chain_levels; ++lev) {
-        const int steps = m.chain_level_len[lev];
-        const bool mine = ch.level == lev;
-        for (int i = 0; i < steps; ++i) {
-            if (!mine || i >= ch.len) continue;
+        const int n = ch.level == lev ? ch.len : 0;     // links this lane walks in this level
+        for (int i = 0; i < n; ++i) {
             const int j = (int)(ch.links >> (5 * i)) & 31;
             double* sl = xs + X_LNK + j * kLinkStride;
             double v[NV];
@@ -693,7 +692,7 @@ __device__ __forceinline__ void chain_inward(double* xs, const ChainC& ch, int l
                 double uu = sl[LK_TAU] - (v[6] + s1 * v[7] + s2 * v[8]);
                 uu -= lm.x;
                 Dj += dt * lm.y;
-                const double dinv = 1.0 / Dj;
+                const double dinv = rcp_pivot(Dj);
                 // Ia = IA - U U^T / D ;  pa = pA + Ia c + U u / D
                 const double n0 = v[0] - U0 * U0 * dinv, n1 = v[1] - U0 * U1 * dinv, n2 = v[2] - U0 * U2 * dinv;
                 const double n3 = v[3] - U1 * U1 * dinv, n4 = v[4] - U1 * U2 * dinv, n5 = v[5] - U2 * U2 * dinv;
@@ -711,7 +710,7 @@ __device__ __forceinline__ void chain_inward(double* xs, const ChainC& ch, int l
                 if (!kElim) store_vals(sl, v);
             }
         }
-        if (mine) store_vals(xs + X_CHO + lane * kChainStride, a);
+        if (n > 0) store_vals(xs + X_CHO + lane * kChainStride, a);
         __syncwarp();
     }
 }
@@ -721,12 +720,10 @@ __device__ __forceinline__ void chain_inward(double* xs, const ChainC& ch, int l
 __device__ __forceinline__ void chain_outward(double* xs, const ChainC& ch, double a0, double a1, double a2) {
     const ModelConst& m = c_model;
     for (int lev = m.chain_levels - 1; lev >= 0; --lev) {
-        const int steps = m.chain_level_len[lev];
-        const bool mine = ch.level == lev;
+        const int n = ch.level == lev ? ch.len : 0;     // links this lane walks in this level, top link first
         double aw = 0.0, alx = 0.0, aly = 0.0;
-        for (int i = 0; i < steps; ++i) {
-            if (!mine || i >= ch.len) continue;
-            const int j = (int)(ch.links >> (5 * (ch.len - 1 - i))) & 31;
+        for (int i = 0; i < n; ++i) {
+            const int j = (int)(ch.links >> (5 * (n - 1 - i))) & 31;
             double* sl = xs + X_LNK + j * kLinkStride;
             if (j == 0) {
                 aw = a0; alx = a1; aly = a2;
@@ -773,9 +770,9 @@ __device__ __forceinline__ void chain_aba(double* xs, const ChainC& ch, int lane
         const double a = shf(ia[0], 0), bx = shf(ia[1], 0), by = shf(ia[2], 0), cxx = shf(ia[3], 0), cxy = shf(ia[4], 0), cyy = shf(ia[5], 0);
         const double r0 = -shf(ia[6], 0), r1 = -shf(ia[7], 0), r2 = -shf(ia[8], 0);
 #endif
-        const double i0 = 1.0 / a, l10 = bx * i0, l20 = by * i0;
-        const double d1 = cxx - l10 * bx, i1 = 1.0 / d1, t21 = cxy - l20 * bx, l21 = t21 * i1;
-        const double d2 = cyy - l20 * by - l21 * t21, i2 = 1.0 / d2;
+        const double i0 = rcp_pivot(a), l10 = bx * i0, l20 = by * i0;
+        const double d1 = cxx - l10 * bx, i1 = rcp_pivot(d1), t21 = cxy - l20 * bx, l21 = t21 * i1;
+        const double d2 = cyy - l20 * by - l21 * t21, i2 = rcp_pivot(d2);
         const double y0 = r0, y1 = r1 - l10 * y0, y2 = r2 - l20 * y0 - l21 * y1;
         a2 = y2 * i2; a1 = y1 * i1 - l21 * a2; a0 = y0 * i0 - l10 * a1 - l20 * a2;
     }
