@@ -384,8 +384,10 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0,
     const int cid = blockIdx.x / kFcCluster, ncl = gridDim.x / kFcCluster;
     if (kTrain && ft.gate && *ft.gate == 0) return;
     const int count = kTrain ? ft.rows : B.pending_count[list];
+    // the slot build reads the settings of each chunk's slot where it decides (ex_dev is the handle's table of kMaxPolicySlots
+    // entries); the single-policy kernel reads entry 0 once
     ExpSettings ex{};
-    if (!kTrain) ex = *ex_dev;
+    if (!kTrain && !kSlots) ex = *ex_dev;
     const int n_char = kTrain ? ft.S - 200 : m.n_char, ncat = kTip0Out + n_char;
     const bool has_net = kTrain || m.has_net;
     const int n_frags = kTrain ? ft.n_frags : m.n_frags, frag = kTrain ? ft.frag : m.frag;
@@ -637,7 +639,7 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0,
         }
         // ---------------- the scalar decisions of this chunk, one lane each
         if (!kTrain && rank == 0 && tid < rows) {
-            if (kSlots) decide_one<true>(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride, W.out_scale + n_frags);
+            if (kSlots) decide_one<true>(B, ex_dev[slot], B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride, W.out_scale + n_frags);
             else decide_one(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride);
         }
         stamp();         // 12: decisions applied
@@ -659,7 +661,7 @@ trl_decide_fc_kernel(Buffers B, NetWeights W, const ExpSettings* __restrict__ ex
     const FwdTrain none{};
     fc_stage<false>(B, W, ex_dev, maps, none, done_count, list, rearm);
 }
-// slot build: chunks from the table of trl_slot_sort_kernel, weights of each chunk's slot
+// slot build: chunks from the table of trl_slot_sort_kernel, weights and exploration settings (ex_dev[slot]) of each chunk's slot
 __global__ void __cluster_dims__(kFcCluster, 1, 1) __launch_bounds__(kFcThreads, 1)
 trl_decide_fc_slots_kernel(Buffers B, PolicySlots P, const ExpSettings* __restrict__ ex_dev, const TRL_GRID_CONSTANT FcMaps maps,
                            const TRL_GRID_CONSTANT FcSlotMaps smaps, const int* __restrict__ tab, int* done_count, int list, int rearm) {

@@ -21,7 +21,10 @@ struct trl_handle {
     int device = 0, n = 0, mode = 0;
     trl::ScenePack scene;
     trl::ModelConst mc;
-    trl::ExpSettings ex;                      // host copy; the kernels read the device copy d_ex
+    // exploration settings per policy slot (trl_set_explore writes every entry, trl_set_explore_slot one).  Host copy; the kernels read
+    // the device table d_ex: the single-policy kernels entry 0, the slot build the entry of each chunk's slot.  `noise` is the same in
+    // every entry (the scene's exploration noise std)
+    trl::ExpSettings ex[trl::kMaxPolicySlots];
     trl::ExpSettings* d_ex = nullptr;
     trl::Buffers B;
     trl::NetWeights W{};

@@ -352,7 +352,7 @@ static int fill_model(trl_handle* h, uint64_t rng_seed) {
         const char* vc = std::getenv("TRL_VERTEX_CONTACTS");
         m.phys = PhysParams{2.0e5, 2.0e3, 0.81, 0.01, 0.00025, 2.0e4, 20.0, (vc && vc[0] == '1') ? 1 : 0};
     }
-    h->ex = ExpSettings{h->mode == TRL_MODE_EXPLORE ? 1 : 0, mf[4], mf[5], mf[6], m.exp_noise};   // uploaded by create_common
+    for (ExpSettings& e : h->ex) e = ExpSettings{h->mode == TRL_MODE_EXPLORE ? 1 : 0, mf[4], mf[5], mf[6], m.exp_noise};   // uploaded by create_common
     if (m.has_net) {
         const auto& nd = s.i32("net_dims");
         if (nd.size() < 5) return fail("scene pack: net_dims missing");
@@ -753,9 +753,9 @@ static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mo
               ck(dalloc(h, &B.tuple_flags, (size_t)B.tuple_cap), "alloc tf") && ck(dalloc(h, &B.tuple_env, (size_t)B.tuple_cap), "alloc te") &&
               ck(dalloc(h, &B.tuple_count, 1), "alloc tc") && ck(dalloc(h, &B.dist_log, (size_t)B.dist_cap), "alloc dl") &&
               ck(dalloc(h, &B.dist_env, (size_t)B.dist_cap), "alloc de") && ck(dalloc(h, &B.dist_count, 1), "alloc dc") &&
-              ck(dalloc(h, &h->done_count, 1), "alloc done") && ck(dalloc(h, &h->d_ex, 1), "alloc ex");
+              ck(dalloc(h, &h->done_count, 1), "alloc done") && ck(dalloc(h, &h->d_ex, (size_t)kMaxPolicySlots), "alloc ex");
     for (int k = 0; ok && h->mc.has_net && k < h->lag; ++k) ok = ck(dalloc(h, &h->act2[k], n * (size_t)5984), "alloc act2");
-    if (ok) ok = ck(cudaMemcpy(h->d_ex, &h->ex, sizeof(ExpSettings), cudaMemcpyHostToDevice), "upload ex");
+    if (ok) ok = ck(cudaMemcpy(h->d_ex, h->ex, sizeof(h->ex), cudaMemcpyHostToDevice), "upload ex");
     if (!ok) return bail("");
     if (h->mc.has_net) {
         const double* blobs[26];
@@ -905,8 +905,19 @@ int trl_set_explore(trl_handle* h, int enable, double rate, double temp, double 
     if (!h) return fail("trl_set_explore: null handle");
     // the decision kernel reads the settings from device memory, so annealing them every update (cScenarioTrain::CalcExpRate
     // ...) neither re-captures the update graph nor drains the stream: the copy is ordered behind the work already queued
-    h->ex.enable = enable; h->ex.rate = rate; h->ex.temp = temp; h->ex.base_rate = base_rate;
-    CK(cudaMemcpyAsync(h->d_ex, &h->ex, sizeof(ExpSettings), cudaMemcpyHostToDevice, h->stream));
+    for (ExpSettings& e : h->ex) { e.enable = enable; e.rate = rate; e.temp = temp; e.base_rate = base_rate; }
+    CK(cudaMemcpyAsync(h->d_ex, h->ex, sizeof(h->ex), cudaMemcpyHostToDevice, h->stream));
+    return 0;
+}
+// the settings of the envs on policy slot `slot` only (slot 0: also those of every single-policy decision); the same ordering as
+// trl_set_explore.  An entry of a slot that holds no policy yet is kept for the policy it will hold
+int trl_set_explore_slot(trl_handle* h, int slot, int enable, double rate, double temp, double base_rate) {
+    if (!h) return fail("trl_set_explore_slot: null handle");
+    if (slot < 0 || slot >= kMaxPolicySlots)
+        return fail("trl_set_explore_slot: slot " + std::to_string(slot) + " out of range (0.." + std::to_string(kMaxPolicySlots - 1) + ")");
+    ExpSettings& e = h->ex[slot];
+    e.enable = enable; e.rate = rate; e.temp = temp; e.base_rate = base_rate;
+    CK(cudaMemcpyAsync(h->d_ex + slot, &e, sizeof(ExpSettings), cudaMemcpyHostToDevice, h->stream));
     return 0;
 }
 

@@ -1498,23 +1498,21 @@ int trl_train_run_timed(trl_trainer* t, const double* sp, int num_updates, int i
     return rc;
 }
 
-// The trl_train_run loop for k trainers of one handle (slot 0's and / or training slots'), in lock-step: every update applies ONE
-// exploration setting and curriculum blend, those of the schedule at the iterations each trainer has done (the same for all,
-// iters_per_update each per update, counted from 0 in every call).  Per update: the update, then one branch per trainer on its own
-// stream -- its hand-over (its slot's rows of the block, in env order) and iters_per_update replays of its training iteration --,
-// the join, and the block's cursor back to zero.  Each trainer computes what a single-trainer handle fed only its slot's rows computes.
-int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp, int num_updates, int iters_per_update, double time_step) {
-    if (!ts || k < 1) return trl_fail("trl_train_run_slots: need at least one trainer");
-    for (int i = 0; i < k; ++i) {
-        TRL_TRAINER_LIVE(ts[i]);
-        if (ts[i]->h != ts[0]->h) return trl_fail("trl_train_run_slots: the trainers belong to different handles");
-        for (int j = 0; j < i; ++j)
-            if (ts[j] == ts[i]) return trl_fail("trl_train_run_slots: trainer " + std::to_string(i) + " is listed twice");
-        if (ts[i]->async) return trl_fail("trl_train_run_slots: asynchronous trainers are not run in lock-step");
-    }
-    if (iters_per_update <= 0) return trl_fail("trl_train_run_slots: iters_per_update must be positive (the trainers advance in lock-step)");
+// The trl_train_run loop for k trainers of one handle (slot 0's and / or training slots'), shared by trl_train_run_slots and
+// trl_train_run_slots_sched.  Per update: the exploration settings and curriculum blend of the schedule, the update, then one branch
+// per trainer on its own stream -- its hand-over (its slot's rows of the block, in env order) and its replays of the training
+// iteration --, the join, and the block's cursor back to zero.  Each trainer computes what a single-trainer handle fed only its
+// slot's rows computes.
+//   per_slot = false: ONE schedule `sp` applied handle-wide (trl_set_explore); iters_per_update > 0.
+//   per_slot = true:  trainer i follows sp + 9 i on its own slot's entry (trl_set_explore_slot).
+//   iters_per_update > 0: lock-step, every trainer's schedule position counts the iterations requested in this call (from 0).
+//   iters_per_update == 0: train_run_impl's pacing per trainer: the schedule at the trainer's iteration counter at the start of the
+//   update, then k_i = (fresh tuples + carry) / tuple_buffer_size iterations.  The counters of all k trainers come back in one round
+//   trip at the start of the update and one after the hand-overs, so the iterations need a second fork behind the first join.
+// The caller has checked the curricula: every trainer sees the same phase at every update, so the blend is trainer 0's.
+static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const double* sp, bool per_slot, int num_updates,
+                          int iters_per_update, int tuple_buffer_size, double time_step) {
     trl_handle* h = ts[0]->h;
-    if (h->comm) return trl_fail("trl_train_run_slots: the handle has a communicator (multi-GPU training runs through trl_train_run)");
     for (int i = 0; i < k; ++i) {
         trl_trainer* t = ts[i];
         if (!t->own_stream) {
@@ -1522,34 +1520,123 @@ int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp, int num
             TCK(cudaEventCreateWithFlags(&t->ev_own, cudaEventDisableTiming));
         }
     }
+    const bool paced = iters_per_update == 0;
+    Counters* hc = nullptr;            // pinned: the k trainers' counters, one synchronisation per read-back
+    if (paced) TCK(cudaMallocHost(&hc, (size_t)k * sizeof(Counters)));
+    auto read_counters = [&]() -> int {
+        for (int i = 0; i < k; ++i) TCK(cudaMemcpyAsync(hc + i, ts[i]->d.c, sizeof(Counters), cudaMemcpyDeviceToHost, h->stream));
+        TCK(cudaStreamSynchronize(h->stream));      // every trainer's stream was joined into the handle's
+        return 0;
+    };
     cudaEvent_t fork;
     TCK(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
-    int rc = 0;
-    long long iters = 0;
-    double last_phase = -1.0;
-    for (int u = 0; u < num_updates && rc == 0; ++u) {
-        double s[4];
-        trl_train_schedule(sp, (int)std::min<long long>(iters, 2000000000LL), s);
-        if (trl_set_explore(h, 1, s[0], s[1], s[2])) { rc = 1; break; }
-        if (s[3] != last_phase) { if (trl_set_terrain_lerp(h, s[3])) { rc = 1; break; } last_phase = s[3]; }
-        if (trl_update(h, time_step)) { rc = 1; break; }
+    auto branch = [&](auto&& body) {
         cudaEventRecord(fork, h->stream);
+        int rc = 0;
         for (int i = 0; i < k && rc == 0; ++i) {
             trl_trainer* t = ts[i];
             cudaStreamWaitEvent(t->own_stream, fork, 0);
-            if (h->train_slots) enqueue_add_slot(t, t->own_stream);
-            else enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, nullptr, t->own_stream, h->B.tuple_env);
-            rc = train_on(t, iters_per_update, t->own_stream);
+            rc = body(i, t);
             cudaEventRecord(t->ev_own, t->own_stream);
         }
         for (int i = 0; i < k; ++i) cudaStreamWaitEvent(h->stream, ts[i]->ev_own, 0);
+        return rc;
+    };
+    auto hand_over = [&](int, trl_trainer* t) {
+        if (h->train_slots) enqueue_add_slot(t, t->own_stream);
+        else enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, nullptr, t->own_stream, h->B.tuple_env);
+        return 0;
+    };
+    std::vector<long long> pos(k, 0), last_total(k, -1), carry(k, 0);
+    std::vector<int> iters(k, iters_per_update);
+    int rc = 0;
+    double last_phase = -1.0;
+    for (int u = 0; u < num_updates && rc == 0; ++u) {
+        if (paced) {
+            if ((rc = read_counters())) break;
+            for (int i = 0; i < k; ++i) {
+                pos[i] = hc[i].iter;
+                if (last_total[i] < 0) last_total[i] = hc[i].total;
+            }
+        }
+        double s[4], phase = 0.0;
+        for (int i = 0; i < k && rc == 0; ++i) {
+            trl_train_schedule(per_slot ? sp + 9 * i : sp, (int)std::min<long long>(pos[i], 2000000000LL), s);
+            if (i == 0) phase = s[3];
+            if (!per_slot) { rc = trl_set_explore(h, 1, s[0], s[1], s[2]); break; }
+            rc = trl_set_explore_slot(h, ts[i]->slot, 1, s[0], s[1], s[2]);
+        }
+        if (rc) break;
+        if (phase != last_phase) { if ((rc = trl_set_terrain_lerp(h, phase))) break; last_phase = phase; }
+        if ((rc = trl_update(h, time_step))) break;
+        if (!paced) {
+            rc = branch([&](int i, trl_trainer* t) { hand_over(i, t); return train_on(t, iters_per_update, t->own_stream); });
+        } else {
+            rc = branch(hand_over);
+            if (rc == 0 && (rc = read_counters()) == 0) {
+                for (int i = 0; i < k; ++i) {
+                    const long long fresh = hc[i].total - last_total[i] + carry[i];
+                    last_total[i] = hc[i].total;
+                    iters[i] = (int)(fresh / tuple_buffer_size);
+                    carry[i] = fresh % tuple_buffer_size;
+                }
+                rc = branch([&](int i, trl_trainer* t) { return iters[i] > 0 ? train_on(t, iters[i], t->own_stream) : 0; });
+            }
+        }
         cudaMemsetAsync(h->B.tuple_count, 0, 4, h->stream);      // cScenarioExp::ResetTupleBuffer, once every trainer has taken its rows
-        iters += iters_per_update;
+        for (int i = 0; i < k; ++i) pos[i] += iters[i];
         const cudaError_t e = cudaGetLastError();
-        if (rc == 0 && e != cudaSuccess) rc = trl_fail(std::string("trl_train_run_slots: ") + cudaGetErrorString(e));
+        if (rc == 0 && e != cudaSuccess) rc = trl_fail(std::string(who) + ": " + cudaGetErrorString(e));
     }
     cudaEventDestroy(fork);
+    if (hc) cudaFreeHost(hc);
     return rc;
+}
+
+// what both entries refuse, with the handle unchanged
+static int check_slot_trainers(const char* who, trl_trainer* const* ts, int k) {
+    const std::string w(who);
+    if (!ts || k < 1) return trl_fail(w + ": need at least one trainer");
+    for (int i = 0; i < k; ++i) {
+        TRL_TRAINER_LIVE(ts[i]);
+        if (ts[i]->h != ts[0]->h) return trl_fail(w + ": the trainers belong to different handles");
+        for (int j = 0; j < i; ++j)
+            if (ts[j] == ts[i]) return trl_fail(w + ": trainer " + std::to_string(i) + " is listed twice");
+        if (ts[i]->async) return trl_fail(w + ": asynchronous trainers are not run in lock-step");
+    }
+    return 0;
+}
+
+// k trainers in lock-step under ONE schedule, applied handle-wide
+int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp, int num_updates, int iters_per_update, double time_step) {
+    if (check_slot_trainers("trl_train_run_slots", ts, k)) return 1;
+    if (iters_per_update <= 0) return trl_fail("trl_train_run_slots: iters_per_update must be positive (the trainers advance in lock-step)");
+    if (ts[0]->h->comm) return trl_fail("trl_train_run_slots: the handle has a communicator (multi-GPU training runs through trl_train_run)");
+    return run_slots_impl("trl_train_run_slots", ts, k, sp, false, num_updates, iters_per_update, 32, time_step);
+}
+
+// k trainers, each under its own schedule sp + 9 i on its own slot's exploration entry; lock-step (iters_per_update > 0) or each paced
+// by its own fresh tuples (iters_per_update == 0, one iteration per tuple_buffer_size)
+int trl_train_run_slots_sched(trl_trainer* const* ts, int k, const double* sp, int num_updates, int iters_per_update, int tuple_buffer_size,
+                              double time_step) {
+    const char* who = "trl_train_run_slots_sched";
+    if (check_slot_trainers(who, ts, k)) return 1;
+    if (!sp) return trl_fail(std::string(who) + ": no schedules");
+    if (iters_per_update < 0) return trl_fail(std::string(who) + ": iters_per_update must be positive, or 0 for one iteration per tuple_buffer_size tuples");
+    if (iters_per_update == 0 && tuple_buffer_size < 1) return trl_fail(std::string(who) + ": tuple_buffer_size must be positive when the trainers are paced by tuples");
+    if (ts[0]->h->comm) return trl_fail(std::string(who) + ": the handle has a communicator (multi-GPU training runs through trl_train_run)");
+    // one terrain blend per update for the whole handle: every trainer must be at the same curriculum phase at every update
+    bool all_off = true, same = true;
+    for (int i = 0; i < k; ++i) {
+        all_off = all_off && sp[9 * i + 8] < 1;
+        same = same && sp[9 * i + 8] == sp[8];
+    }
+    if (iters_per_update == 0 && !all_off)
+        return trl_fail(std::string(who) + ": trainers paced by tuples reach different curriculum phases (the handle has one terrain blend): "
+                        "every trainer_curriculum_iters must be < 1");
+    if (!all_off && !same)
+        return trl_fail(std::string(who) + ": the schedules differ in trainer_curriculum_iters (the handle has one terrain blend per update)");
+    return run_slots_impl(who, ts, k, sp, true, num_updates, iters_per_update, tuple_buffer_size, time_step);
 }
 
 // c[9]: iter, actor_iter, stage, num, head, total, critic buffer, actor buffer, pending actor batch; l[2]: last losses

@@ -132,6 +132,7 @@ EXPORTS = [
     "trl_load_policy", "trl_set_env_policy", "trl_eval_stats_slot",
     "trl_load_terrain", "trl_set_env_terrain", "trl_env_terrain", "trl_eval_stats_cell",
     "trl_trainer_create_slot", "trl_train_run_slots", "trl_output_model_slot",
+    "trl_set_explore_slot", "trl_train_run_slots_sched",
 ]
 
 
@@ -455,8 +456,13 @@ class ScenarioExpMACE(BatchedScenario):
     """cScenarioExpMACE over a batch (scenarios/ScenarioExp.h:16-40, ScenarioExpMACE.h)."""
     MODE = 1
 
-    def EnableExplore(self, enable, rate, temp, base_rate):
-        self._ck(self.L.trl_set_explore(self.h, int(enable), C.c_double(rate), C.c_double(temp), C.c_double(base_rate)))
+    def EnableExplore(self, enable, rate, temp, base_rate, slot=None):
+        """the exploration settings of every env, or (slot = p) only of the envs on policy slot p"""
+        if slot is None:
+            self._ck(self.L.trl_set_explore(self.h, int(enable), C.c_double(rate), C.c_double(temp), C.c_double(base_rate)))
+        else:
+            self._ck(self.L.trl_set_explore_slot(self.h, int(slot), int(enable), C.c_double(rate), C.c_double(temp),
+                                                 C.c_double(base_rate)))
 
     def GetNumTuples(self):
         n = C.c_int(0)

@@ -131,18 +131,34 @@ class ScenarioTrainMACE:
         self.exp.OutputModel(path, mtime=int(time.time()))            # native writer behind the C ABI (csrc/model_io.h)
 
 
-def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step=1.0 / 30.0):
-    """cScenarioTrain::Run for several trainers of one exploration scenario (trl_train_run_slots): `num_updates` updates of the
-    whole batch, each followed by every trainer's hand-over of its slot's tuples and `iters_per_update` iterations, the trainers side by
-    side on their own streams.  The exploration settings and curriculum blend follow `schedule` at the iterations each trainer has done
-    in this call (the same for all)."""
+def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step=1.0 / 30.0, tuple_buffer_size=32):
+    """cScenarioTrain::Run for several trainers of one exploration scenario: `num_updates` updates of the whole batch, each followed
+    by every trainer's hand-over of its slot's tuples and its iterations, the trainers side by side on their own streams.
+
+    schedule: one TrainSchedule for all trainers, or a list with one per trainer (each applied to its own slot's envs).
+    iters_per_update: the iterations of every trainer per update (lock-step; the schedules are read at the iterations done in this
+    call); None = each trainer paced as in ScenarioTrainMACE: one iteration per `tuple_buffer_size` fresh tuples of its slot, its
+    schedule read at its own iteration count.  One schedule with a fixed count is trl_train_run_slots (applied handle-wide); every
+    other call is trl_train_run_slots_sched."""
     trainers = list(trainers)
     if not trainers:
         raise ValueError("train_run_slots: no trainer")
     L = trainers[0].L
     arr = (C.c_void_p * len(trainers))(*[t.h.value if t.h is not None else None for t in trainers])
-    sp = np.array([schedule.p[k] for k in TrainSchedule.KEYS], float)
-    rc = L.trl_train_run_slots(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), int(iters_per_update),
-                               C.c_double(time_step))
+    per_trainer = isinstance(schedule, (list, tuple))
+    if not per_trainer and iters_per_update is not None:
+        sp = np.array([schedule.p[k] for k in TrainSchedule.KEYS], float)
+        rc = L.trl_train_run_slots(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), int(iters_per_update),
+                                   C.c_double(time_step))
+    else:
+        scheds = list(schedule) if per_trainer else [schedule] * len(trainers)
+        if len(scheds) != len(trainers):
+            raise ValueError("train_run_slots: %d schedules for %d trainers" % (len(scheds), len(trainers)))
+        if iters_per_update is not None and int(iters_per_update) <= 0:
+            raise ValueError("train_run_slots: iters_per_update must be positive, or None for tuple pacing")
+        sp = np.array([[s.p[k] for k in TrainSchedule.KEYS] for s in scheds], float)
+        rc = L.trl_train_run_slots_sched(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates),
+                                         0 if iters_per_update is None else int(iters_per_update), int(tuple_buffer_size),
+                                         C.c_double(time_step))
     if rc != 0:
         raise RuntimeError(L.trl_last_error().decode())

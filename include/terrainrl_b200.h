@@ -52,8 +52,14 @@ int trl_update(trl_handle* h, double dt);
 int trl_env_step(trl_handle* h, double step);
 int trl_sync(trl_handle* h);
 
-/* cScenarioExp::{EnableExplore,SetExpRate,SetExpTemp,SetExpBaseActionRate}   scenarios/ScenarioExp.cpp:156-185 */
+/* cScenarioExp::{EnableExplore,SetExpRate,SetExpTemp,SetExpBaseActionRate}   scenarios/ScenarioExp.cpp:156-185
+ *   trl_set_explore       the settings of every env (every policy slot's entry)
+ *   trl_set_explore_slot  the settings of the envs on policy slot `slot` (0..7) only; slot 0's entry is also the one a handle
+ *                         without policy slots uses.  A slot that holds no policy yet keeps its entry until it does.  Refused for a
+ *                         slot out of range.  The exploration noise std stays the scene's, for every slot.
+ * Both are ordered on the handle's stream behind the work already queued; neither drains it. */
 int trl_set_explore(trl_handle* h, int enable, double rate, double temp, double base_rate);
+int trl_set_explore_slot(trl_handle* h, int slot, int enable, double rate, double temp, double base_rate);
 /* engine contact / joint-limit parameters (7 doubles: kn, dn, mu, v_eps, contact_tol, k_lim, d_lim) */
 int trl_set_phys_params(trl_handle* h, const double* p7);
 
@@ -251,11 +257,21 @@ int trl_trainer_rows(trl_trainer* t, const int32_t* slots, int n, float* rows, i
  *   trl_train_run_slots  the trl_train_run loop for k trainers of one handle in lock-step (iters_per_update > 0 each per update,
  *                        one exploration setting and curriculum blend per update, annealed from 0 in every call).  Refused for
  *                        trainers of different handles, a trainer listed twice, k < 1 and iters_per_update <= 0.
+ *   trl_train_run_slots_sched  the same loop with a schedule per trainer: trainer i anneals by sp9[9 i .. 9 i + 9) and applies the
+ *                        result to its own slot (trl_set_explore_slot); slots of unlisted trainers keep their entries.
+ *                        iters_per_update > 0: lock-step, annealed from 0 in every call.  iters_per_update == 0: each trainer paced
+ *                        as trl_train_run(t, sp, U, 0, tuple_buffer_size, dt) paces it: the schedule at its iteration counter at the
+ *                        start of the update, one iteration per tuple_buffer_size fresh tuples of its slot, the remainder carried.
+ *                        The handle keeps one terrain blend per update: refused unless every schedule has the same
+ *                        trainer_curriculum_iters or all have it < 1 (paced: all < 1).  Also refused for whatever
+ *                        trl_train_run_slots refuses, iters_per_update < 0 and, paced, tuple_buffer_size < 1.
  * Once a handle has a training slot: trl_trainer_add_from_scene hands a trainer only its slot's tuples and leaves the block to the
  * others (trl_reset_tuples clears it); trl_set_env_policy is refused while the block holds tuples and resets the envs it moves, so
  * every tuple belongs to the slot that chose its action; trl_train_run / trl_train_run_timed / trl_trainer_set_async are refused. */
 trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* params10, const char* h5_path, const char* scale_json_path);
 int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp9, int num_updates, int iters_per_update, double time_step);
+int trl_train_run_slots_sched(trl_trainer* const* ts, int k, const double* sp9k, int num_updates, int iters_per_update, int tuple_buffer_size,
+                              double time_step);
 
 /* number of tuples the engine could not record because the tuple block was full (cScenarioExp's ring overwrites, scenarios/
  * ScenarioExp.cpp:296-301; a batch block refuses instead and counts).  trl_num_tuples / trl_get_tuples* return
