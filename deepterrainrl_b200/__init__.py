@@ -10,3 +10,4 @@ from .scenario import (BatchedScenario, ScenarioExpMACE, ScenarioPoliEval, build
 
 __all__ = ["BatchedScenario", "ScenarioExpMACE", "ScenarioPoliEval", "build_library", "library_path", "load_library", "pack_from_args"]
 from .trainer import MACETrainer  # noqa: F401,E402
+from .checkpoint import load_checkpoint  # noqa: F401,E402

@@ -4,6 +4,8 @@
 #pragma once
 #include <cstdint>
 #include <fstream>
+#include <istream>
+#include <ostream>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -15,15 +17,21 @@ public:
     bool load(const std::string& path, std::string* err) {
         std::ifstream in(path, std::ios::binary);
         if (!in) { if (err) *err = "cannot open scene pack: " + path; return false; }
+        return read(in, path, err);
+    }
+    // a pack from a stream positioned at its magic that holds nothing after it (the scene section of a checkpoint); `path` names it in
+    // the messages
+    bool read(std::istream& in, const std::string& path, std::string* err) {
         char magic[8];
         in.read(magic, 8);
         if (!in || std::string(magic, 8) != "TRLPACK1") { if (err) *err = "not a TRLPACK1 file: " + path; return false; }
         uint32_t count = 0;
         in.read(reinterpret_cast<char*>(&count), 4);
         // every length in the file is checked against what is left of it before anything is allocated
+        const std::streampos body = in.tellg();
         in.seekg(0, std::ios::end);
         const uint64_t file_size = (uint64_t)in.tellg();
-        in.seekg(12, std::ios::beg);
+        in.seekg(body);
         auto remaining = [&]() { return file_size - (uint64_t)in.tellg(); };
         for (uint32_t r = 0; r < count && in; ++r) {
             uint32_t len = 0, dtype = 0;
@@ -68,6 +76,9 @@ public:
     bool save(const std::string& path, std::string* err) const {
         std::ofstream out(path, std::ios::binary);
         if (!out) { if (err) *err = "cannot write " + path; return false; }
+        return write(out);
+    }
+    bool write(std::ostream& out) const {
         out.write("TRLPACK1", 8);
         uint32_t count = (uint32_t)order_.size();
         out.write(reinterpret_cast<const char*>(&count), 4);

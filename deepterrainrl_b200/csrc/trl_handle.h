@@ -109,3 +109,21 @@ int trl_reupload_model(trl_handle* h);                // after editing h->mc: re
 // policy slot `slot` >= 1 gets its own blobs holding the Caffe-HDF5 model + `_scale.txt` (both paths given) or a copy of slot 0's
 // current net, and the handle gets its slot machinery; refused, with nothing changed, for a model of another topology
 extern "C" int trl_stage_slot_model(trl_handle* h, int slot, const char* h5_path, const char* scale_path);
+// the rest of trl_create_from_pack once h->scene is loaded (nullptr, with h deleted and the reason recorded, on failure)
+extern "C" trl_handle* trl_create_common(trl_handle* h, int num_envs, int device, int mode, const uint64_t* terrain_seeds, uint64_t rng_seed);
+int trl_drain(trl_handle* h);                         // every stream of the handle idle
+// terrain slot `slot` >= 1 holds parameter sets [n][40] of generator `type` (trl_load_terrain once the file is read)
+int trl_set_terrain_slot(trl_handle* h, int slot, int type, std::vector<double> sets);
+
+// One array of a checkpoint (trl_checkpoint.cu): `bytes` of device memory at `dev`, or of host memory at `host` when dev is null.
+// `cap` is the room there is: a restore accepts up to cap bytes (the replay rows, the tuple block and the distance log are saved up
+// to their fill level)
+struct CkptSection {
+    std::string name;
+    int dtype;             // 0 raw bytes, 1 i32, 2 f32, 3 f64 (informative)
+    void* dev;
+    void* host;
+    size_t bytes, cap;
+};
+// the sections of a trainer's carried state, named prefix + field (trl_train.cu); drains the trainer, refuses an asynchronous one
+int trl_trainer_state(trl_trainer* t, const std::string& prefix, std::vector<CkptSection>* out);

@@ -643,7 +643,6 @@ extern "C" {
 
 const char* trl_last_error(void) { return g_err.c_str(); }
 
-static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mode, const uint64_t* terrain_seeds, uint64_t rng_seed);
 
 trl_handle* trl_create_from_pack(const char* pack_path, int num_envs, int device, int mode, const uint64_t* terrain_seeds,
                                  uint64_t rng_seed) {
@@ -651,7 +650,7 @@ trl_handle* trl_create_from_pack(const char* pack_path, int num_envs, int device
     try {
         std::string err;
         if (!h->scene.load(pack_path, &err)) { g_err = err; delete h; return nullptr; }
-        return create_common(h, num_envs, device, mode, terrain_seeds, rng_seed);
+        return trl_create_common(h, num_envs, device, mode, terrain_seeds, rng_seed);
     } catch (const std::exception& e) {       // bad_alloc / out_of_range from a damaged pack must not cross the C ABI
         g_err = std::string("trl_create_from_pack: ") + e.what();
         delete h;
@@ -669,7 +668,7 @@ trl_handle* trl_create(int argc, const char* const* argv, const char* data_root,
         delete h;
         return nullptr;
     }
-    return create_common(h, num_envs, device, mode, terrain_seeds, rng_seed);
+    return trl_create_common(h, num_envs, device, mode, terrain_seeds, rng_seed);
 }
 
 int trl_pack_from_args(int argc, const char* const* argv, const char* data_root, const char* out_path) {
@@ -684,7 +683,7 @@ int trl_pack_from_args(int argc, const char* const* argv, const char* data_root,
     return 0;
 }
 
-static trl_handle* create_common(trl_handle* h, int num_envs, int device, int mode, const uint64_t* terrain_seeds, uint64_t rng_seed) {
+trl_handle* trl_create_common(trl_handle* h, int num_envs, int device, int mode, const uint64_t* terrain_seeds, uint64_t rng_seed) {
     auto bail = [&](const std::string& why) -> trl_handle* {
         if (!why.empty()) g_err = why;
         trl_destroy(h);
@@ -1140,19 +1139,7 @@ int trl_load_terrain(trl_handle* h, int slot, const char* terrain_json_path) {
     } catch (const std::exception& e) {
         return fail(std::string("trl_load_terrain: ") + e.what());
     }
-    TerrainSlot ts{};
-    ts.type = tf.type;
-    blend_terrain(tf.params.data(), tf.n_sets, h->scene.f64("terrain_default_params").data(), h->terrain_lerp, ts.params);
-    if (drain(h)) return 1;
-    if (h->env_terrain_host.empty()) {     // first slot: from now on the step launches run the terrain-slot build
-        h->env_terrain_host.assign((size_t)h->n, 0);
-        destroy_graphs(h);
-    }
-    h->terrain_sets[slot] = std::move(tf.params);
-    h->terrain_loaded[slot] = true;
-    h->terrain[slot] = ts;
-    g_model_owner = nullptr;
-    return ensure_model(h) ? fail("trl_load_terrain: terrain table upload failed") : 0;
+    return trl_set_terrain_slot(h, slot, tf.type, std::move(tf.params));
 }
 
 int trl_set_env_terrain(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
@@ -1181,6 +1168,13 @@ int trl_env_terrain(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
     const size_t N = (size_t)h->n;
     if (current && n > 0) CK(cudaMemcpy(current, h->B.i + (size_t)I_TERRAIN_SLOT * N, (size_t)n * 4, cudaMemcpyDeviceToHost));
     if (assigned && n > 0) CK(cudaMemcpy(assigned, h->B.i + (size_t)I_TERRAIN_SLOT_NEXT * N, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+// the policy slot of envs 0 .. n-1 (all 0 while only slot 0 exists)
+int trl_env_policy(trl_handle* h, int32_t* slots, int n) {
+    if (!h) return fail("trl_env_policy: null handle");
+    if (n < 0 || n > h->n) return fail("trl_env_policy: env count out of range");
+    for (int k = 0; k < n; ++k) slots[k] = h->slots_active ? h->env_slot_host[k] : 0;
     return 0;
 }
 int trl_get_output_offset_scale(trl_handle* h, double* off, double* scale, int n);
@@ -1873,3 +1867,21 @@ static int update_timed_impl(trl_handle* h, double dt, double* step_ms, int* ste
 }
 
 }  // extern "C"
+
+int trl_drain(trl_handle* h) { return drain(h); }
+
+int trl_set_terrain_slot(trl_handle* h, int slot, int type, std::vector<double> sets) {
+    TerrainSlot ts{};
+    ts.type = type;
+    blend_terrain(sets.data(), (int)(sets.size() / kTerrainParams), h->scene.f64("terrain_default_params").data(), h->terrain_lerp, ts.params);
+    if (drain(h)) return 1;
+    if (h->env_terrain_host.empty()) {     // first slot: from now on the step launches run the terrain-slot build
+        h->env_terrain_host.assign((size_t)h->n, 0);
+        destroy_graphs(h);
+    }
+    h->terrain_sets[slot] = std::move(sets);
+    h->terrain_loaded[slot] = true;
+    h->terrain[slot] = ts;
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail("trl_load_terrain: terrain table upload failed") : 0;
+}

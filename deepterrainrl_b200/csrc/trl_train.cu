@@ -27,6 +27,7 @@
 #include "../../include/terrainrl_b200.h"
 #include "trl_handle.h"
 #include "trl_comm.h"
+#include "trl_mix64.h"
 
 namespace trl {
 void launch_forward_train(const NetWeights& W, const FcMaps& maps, const FwdTrain& f, double* act2, cudaStream_t st);
@@ -96,12 +97,6 @@ __device__ __forceinline__ bool pred_on(const Dev& d, int pred) {
         case P_INIT: return d.c->init_now != 0;
         default: return true;
     }
-}
-__device__ __forceinline__ unsigned long long mix64(unsigned long long z) {
-    z += 0x9E3779B97F4A7C15ull;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
 }
 __device__ __forceinline__ int rand_int(const Dev& d, int mn, int mx) {      // cMathUtil::RandInt(min, max), counter RNG
     if (mn == mx) return mn;
@@ -817,6 +812,7 @@ struct trl_trainer {
     int slot = 0;                      // policy slot whose net this trainer is (0: the handle's own, h->trainer)
     cudaStream_t own_stream = nullptr; // trl_train_run_slots: hand-over + iterations of this trainer beside the other trainers'
     cudaEvent_t ev_own = nullptr;
+    double params[10] = {};            // the creation parameters (trl_trainer_create's p[10])
 };
 
 #define TCK(call)                                                                                       \
@@ -1001,16 +997,8 @@ static trl_trainer* trainer_new(trl_handle* h, const double* p) {
     d.A = 1 + m.frag; d.Wd = 1 + d.S + d.A + d.S; d.cat = T + m.n_char;
     d.cap = (int)p[0]; d.nis = (int)p[1]; d.steps_per_iter = std::max(1, (int)p[2]); d.freeze = (int)p[3];
     d.init_offset_scale = (int)p[4]; d.discount = p[5]; d.base_lr = p[6]; d.momentum = p[7]; d.weight_decay = p[8];
-    {
-        // CounterRng::seed(seed, stream) of the engine, stream tag "tran"
-        auto mix = [](unsigned long long z) {
-            z += 0x9E3779B97F4A7C15ull;
-            z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-            z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-            return z ^ (z >> 31);
-        };
-        d.rng_key = mix((unsigned long long)p[9] ^ mix(0x7472616eull));
-    }
+    std::memcpy(t->params, p, sizeof(t->params));
+    d.rng_key = trl::mix64((unsigned long long)p[9] ^ trl::mix64(0x7472616eull));     // CounterRng::seed(seed, stream) of the engine, stream tag "tran"
     if (d.S != kTerr + d.n_char || d.cat > 160 || d.n_out != d.n_frags * (1 + d.frag) || d.cap < 2 * kB) {
         trl_fail("trl_trainer_create: unsupported net dimensions / replay capacity");
         delete t;
@@ -1698,4 +1686,44 @@ int trl_trainer_list(trl_trainer* t, int which, int32_t* out, int cap, int* len)
     return 0;
 }
 
+// the creation parameters p[10] of trl_trainer_create and the policy slot the trainer trains
+int trl_trainer_params(trl_trainer* t, double* params10, int* slot) {
+    TRL_TRAINER_LIVE(t);
+    if (params10) std::memcpy(params10, t->params, sizeof(t->params));
+    if (slot) *slot = t->slot;
+    return 0;
+}
+
 }  // extern "C"
+
+// A new field of Dev or Counters is either state a checkpoint carries (list it below) or scratch one Train() rewrites before reading it:
+// these sizes make the decision explicit
+static_assert(sizeof(Counters) == 88, "Counters changed: update trl_trainer_state");
+static_assert(sizeof(Dev) == 568, "Dev changed: update trl_trainer_state");
+
+// What carries from one call on the trainer to the next (trl_checkpoint.cu), after its streams have drained: the current and target nets
+// with their offset / scale vectors, the momentum history, replay rows [0, num) and their flags, the critic / actor buffers with their
+// position tables, the pending actor batch, the ids of the last sampled batch (trl_trainer_list 3), the counter block and the RNG key.
+// Not carried: the gradient, activations, candidates, labels, column means (each Train() writes them before it reads them) and the
+// hand-over scratch.  An asynchronous trainer has a job in flight across updates and is refused.
+int trl_trainer_state(trl_trainer* t, const std::string& prefix, std::vector<CkptSection>* out) {
+    TRL_TRAINER_LIVE(t);
+    if (t->async) return trl_fail("trl_checkpoint_save: the trainer of slot " + std::to_string(t->slot) + " is asynchronous");
+    TCK(trainer_sync(t));
+    Dev& d = t->d;
+    Counters c;
+    TCK(cudaMemcpy(&c, d.c, sizeof(c), cudaMemcpyDeviceToHost));
+    const size_t P = (size_t)d.P * 8, S = (size_t)d.S * 8, O = (size_t)d.n_out * 8, cap = (size_t)d.cap, num = (size_t)c.num;
+    auto fixed = [&](const char* name, int dtype, void* p, size_t bytes) { out->push_back(CkptSection{prefix + name, dtype, p, nullptr, bytes, bytes}); };
+    fixed("theta", 3, d.theta, P); fixed("target", 3, d.target, P); fixed("history", 3, d.history, P);
+    fixed("in_off", 3, d.in_off, S); fixed("in_scale", 3, d.in_scale, S); fixed("out_off", 3, d.out_off, O); fixed("out_scale", 3, d.out_scale, O);
+    fixed("t_in_off", 3, d.t_in_off, S); fixed("t_in_scale", 3, d.t_in_scale, S); fixed("t_out_off", 3, d.t_out_off, O); fixed("t_out_scale", 3, d.t_out_scale, O);
+    out->push_back(CkptSection{prefix + "mem", 2, d.mem, nullptr, num * d.Wd * 4, cap * d.Wd * 4});
+    out->push_back(CkptSection{prefix + "flags", 1, d.flags, nullptr, num * 4, cap * 4});
+    fixed("pos_critic", 1, d.pos_critic, cap * 4); fixed("pos_actor", 1, d.pos_actor, cap * 4);
+    fixed("critic_list", 1, d.critic_list, cap * 4); fixed("actor_list", 1, d.actor_list, cap * 4);
+    fixed("actor_batch", 1, d.actor_batch, 4 * trl_train::kB * 4); fixed("ids", 1, d.ids, trl_train::kB * 4);
+    fixed("counters", 0, d.c, sizeof(Counters));
+    out->push_back(CkptSection{prefix + "rng_key", 0, nullptr, &d.rng_key, 8, 8});
+    return 0;
+}

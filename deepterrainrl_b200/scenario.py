@@ -84,7 +84,7 @@ def build_library(force=False, verbose=False):
     out = library_path()
     csrc = os.path.join(_PKG, "csrc")
     units = [("trl_step.cu", []), ("trl_step_cg.cu", ["-Xptxas", "-dlcm=cg"]), ("trl_step_ts.cu", []), ("trl_step_ts_cg.cu", ["-Xptxas", "-dlcm=cg"]),
-             ("trl_host.cu", []), ("trl_train.cu", []),
+             ("trl_host.cu", []), ("trl_train.cu", []), ("trl_checkpoint.cu", []),
              ("trl_comm.cu", []), ("trl_probe.cu", []), ("trl_tc_policy.cu", []), ("ref_loader.cpp", [])]
     deps = [os.path.join(csrc, f) for f in os.listdir(csrc)]
     deps.append(os.path.join(_ROOT, "include", "terrainrl_b200.h"))
@@ -133,6 +133,7 @@ EXPORTS = [
     "trl_load_terrain", "trl_set_env_terrain", "trl_env_terrain", "trl_eval_stats_cell",
     "trl_trainer_create_slot", "trl_train_run_slots", "trl_output_model_slot",
     "trl_set_explore_slot", "trl_train_run_slots_sched",
+    "trl_checkpoint_save", "trl_create_from_checkpoint", "trl_trainer_params", "trl_env_policy",
 ]
 
 
@@ -185,6 +186,17 @@ class BatchedScenario:
                                             C.c_uint64(rng_seed))
         if not h:
             raise RuntimeError("trl_create: " + self.L.trl_last_error().decode())
+        self._attach(h)
+
+    @classmethod
+    def _wrap(cls, L, h):
+        """a scenario object over a handle the library has already created (load_checkpoint)"""
+        obj = cls.__new__(cls)
+        obj.L = L
+        obj._attach(h)
+        return obj
+
+    def _attach(self, h):
         self.h = C.c_void_p(h)
         v = [C.c_int(0) for _ in range(7)]
         self._ck(self.L.trl_sizes(self.h, *[C.byref(x) for x in v]))
@@ -222,6 +234,12 @@ class BatchedScenario:
             self._ck(self.L.trl_output_model(self.h, path.encode(), C.c_uint32(mtime)))
         else:
             self._ck(self.L.trl_output_model_slot(self.h, int(slot), path.encode(), C.c_uint32(mtime)))
+
+    def SaveCheckpoint(self, path, user=b""):
+        """everything a later call on this scenario and its trainers reads, to `path` (trl_checkpoint_save), with the bytes `user`
+        stored verbatim; deepterrainrl_b200.load_checkpoint resumes it bit for bit in another process.  The scenario is unchanged."""
+        user = bytes(user)
+        self._ck(self.L.trl_checkpoint_save(self.h, os.fspath(path).encode(), user, C.c_size_t(len(user))))
 
     def LoadModel(self, h5_path, scale_path=None):
         """cNeuralNet::LoadModel + LoadScale from the reference's file formats."""

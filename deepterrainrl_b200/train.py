@@ -9,6 +9,7 @@ iterations on the GPU, and the annealed exploration settings for the next update
 iterations per update is a parameter here (`iters_per_update`; None = one iteration per tuple_buffer_size new tuples, read back
 from the device once per update)."""
 import ctypes as C
+import json
 import os
 
 import numpy as np
@@ -123,6 +124,31 @@ class ScenarioTrainMACE:
                 self.OutputModel(self.output_path)
             if self.trainer.params and self._iters >= self.max_iter:
                 break
+
+    # the loop's own state, stored in a checkpoint's user blob
+    _LOOP_STATE = ("iters_per_update", "tuple_buffer_size", "iters_per_output", "output_path", "max_iter", "time_step", "_iters",
+                   "_last_total", "_carry")
+
+    def Checkpoint(self, path):
+        """the scenario, its trainer and this loop's state to `path`: resume(path) continues the run as if it had never stopped"""
+        state = {k: getattr(self, k) for k in self._LOOP_STATE}
+        state["schedule"] = self.schedule.p
+        self.exp.SaveCheckpoint(path, json.dumps(state).encode())
+
+    @classmethod
+    def resume(cls, path, device=0):
+        """the loop a Checkpoint() wrote, on `device`: Run(N + M) == Run(N); Checkpoint(path); resume(path).Run(M)"""
+        from .checkpoint import load_checkpoint
+        exp, trainers, user = load_checkpoint(path, device)
+        if set(trainers) != {0}:
+            raise RuntimeError(f"{path}: not a checkpoint of ScenarioTrainMACE (trainers on slots {sorted(trainers)})")
+        state = json.loads(user.decode())
+        obj = cls.__new__(cls)
+        obj.schedule = TrainSchedule(**state.pop("schedule"))
+        for k in cls._LOOP_STATE:
+            setattr(obj, k, state[k])
+        obj.exp, obj.trainer = exp, trainers[0]
+        return obj
 
     def OutputModel(self, path):
         """cNeuralNet::OutputModel (learning/NeuralNet.cpp:571-587, 1182-1205): Caffe-layout HDF5 + `<stem>_scale.txt`."""

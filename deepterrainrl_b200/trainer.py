@@ -38,16 +38,35 @@ class MACETrainer:
         p = dict(self.DEFAULTS)
         p.update(kw)
         self.params = p
-        arr = np.array([p[k] for k in ("replay_mem_size", "num_init_samples", "num_steps_per_iter", "freeze_target_iters",
-                                       "init_input_offset_scale", "discount", "base_lr", "momentum", "weight_decay", "seed")], float)
-        self.scenario = scenario
+        arr = np.array([p[k] for k in self.PARAM_KEYS], float)
         self.slot = int(slot)
         h5, scale = (None, None) if model is None else (os.fspath(model[0]).encode(), os.fspath(model[1]).encode())
         h = L.trl_trainer_create_slot(scenario.h, self.slot, _p(arr), h5, scale)
         if not h:
             raise RuntimeError(L.trl_last_error().decode())
+        self._attach(scenario, h)
+
+    PARAM_KEYS = ("replay_mem_size", "num_init_samples", "num_steps_per_iter", "freeze_target_iters", "init_input_offset_scale",
+                  "discount", "base_lr", "momentum", "weight_decay", "seed")
+
+    @classmethod
+    def _wrap(cls, scenario, h):
+        """a trainer object over a trainer the library has already created (load_checkpoint): parameters and slot as created"""
+        obj = cls.__new__(cls)
+        obj.L = scenario.L
+        p = np.zeros(10)
+        slot = C.c_int(0)
+        if obj.L.trl_trainer_params(C.c_void_p(h), _p(p), C.byref(slot)) != 0:
+            raise RuntimeError(obj.L.trl_last_error().decode())
+        obj.params = {k: (float(v) if k in ("discount", "base_lr", "momentum", "weight_decay") else int(v)) for k, v in zip(cls.PARAM_KEYS, p)}
+        obj.slot = slot.value
+        obj._attach(scenario, h)
+        return obj
+
+    def _attach(self, scenario, h):
+        self.scenario = scenario
         self.h = C.c_void_p(h)
-        self.num_params = L.trl_trainer_num_params(self.h)
+        self.num_params = self.L.trl_trainer_num_params(self.h)
         self.S, self.A = scenario.state_size, scenario.action_size
         self.n_out = scenario.num_frags * (1 + scenario.frag_size)
         self.W = 1 + 2 * self.S + self.A

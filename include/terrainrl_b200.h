@@ -243,6 +243,27 @@ int trl_trainer_get(trl_trainer* t, int what, double* out);
 int trl_trainer_set_theta(trl_trainer* t, const double* theta);
 int trl_trainer_list(trl_trainer* t, int which, int32_t* out, int cap, int* len);
 int trl_trainer_rows(trl_trainer* t, const int32_t* slots, int n, float* rows, int32_t* flags);
+/* the creation parameters params10 of trl_trainer_create and the policy slot the trainer trains (either may be NULL) */
+int trl_trainer_params(trl_trainer* t, double* params10, int* slot);
+
+/* checkpoints: a run stopped between two calls and resumed in another process is the same run.
+ *   trl_checkpoint_save         drains the handle and its trainers' streams, then writes everything a later call reads to `path`
+ *                               (TRLCKPT1: a section table of name, dtype, byte count and device-computed 64-bit digest, then the raw
+ *                               bytes): the scene pack, the env state, the tuple block, the distance log, the exploration settings,
+ *                               the physics parameters, every policy and terrain slot, every trainer with its replay memory, and
+ *                               `user_bytes` of `user` stored verbatim.  Saving changes nothing in the handle.  Refused, with nothing
+ *                               written, for a handle with a communicator, an asynchronous trainer or a pending trl_snapshot.
+ *   trl_create_from_checkpoint  a handle on `device` from such a file with its trainers: trainers[p] (an array of 8, or NULL) is the
+ *                               trainer of policy slot p or NULL; destroy them with trl_trainer_destroy as usual.  The user blob is
+ *                               copied into `user` (up to user_cap bytes; *user_bytes = its full length).  Every later call on the
+ *                               new handle and its trainers returns, bit for bit, what it returns on the handle that saved, under any
+ *                               of the overlapped schedule, the serial schedule or env groups.  NULL on failure (a damaged,
+ *                               truncated or foreign file, a digest mismatch: trl_last_error names the section), with nothing left
+ *                               allocated.
+ *   trl_env_policy              the policy slot of envs 0 .. n-1. */
+int trl_checkpoint_save(trl_handle* h, const char* path, const void* user, size_t user_bytes);
+trl_handle* trl_create_from_checkpoint(const char* path, int device, trl_trainer** trainers, void* user, size_t user_cap, size_t* user_bytes);
+int trl_env_policy(trl_handle* h, int32_t* slots, int n);
 
 /* training slots: one exploration handle (TRL_MODE_EXPLORE) trains up to 8 policies side by side, one trainer per policy slot, each
  * env exploring with the net of its slot (trl_set_env_policy) and feeding that slot's trainer.  Env i on slot p computes exactly what
