@@ -186,6 +186,10 @@ int handle_state(trl_handle* h, std::vector<CkptSection>* out) {
         fixed("env_slot", 1, h->P.env_slot, n * 4);
     }
     if (!h->env_terrain_host.empty()) host("env_terrain_host", 1, h->env_terrain_host.data(), n * 4);
+    if (h->env_phys) {       // physics slots: written only once one is loaded, so a handle without keeps the same file
+        host("env_phys_host", 1, h->env_phys_host.data(), n * 4);
+        fixed("env_phys", 1, h->env_phys, 2 * n * 4);
+    }
     fixed("B.d", 3, B.d, (size_t)D_NUM_FIELDS * n * 8);
     fixed("B.i", 1, B.i, (size_t)I_NUM_PLANES * n * 4);
     fixed("B.terrain", 2, B.terrain, n * 2 * kTerrainCap * 4);
@@ -278,6 +282,13 @@ int save_impl(trl_handle* h, const char* path, const void* user, size_t user_byt
         m.terrains |= 1 << s;
         m.terrain_type[s] = h->terrain[s].type;
         build.push_back(blob_of("terrain_sets." + std::to_string(s), 3, h->terrain_sets[s].data(), h->terrain_sets[s].size()));
+    }
+    if (h->env_phys) {
+        int32_t mask = 0;
+        for (int s = 1; s < kMaxPhysSlots; ++s)
+            if (h->phys_loaded[s]) mask |= 1 << s;
+        build.push_back(blob_of("phys_loaded", 1, &mask, 1));
+        build.push_back(blob_of("phys_table", 0, h->phys, kMaxPhysSlots));
     }
     build.insert(build.begin() + 1, blob_of("meta", 0, &m, 1));
     build.push_back(blob_of("user", 0, (const unsigned char*)user, user_bytes));
@@ -407,6 +418,20 @@ trl_handle* load_impl(const char* path, int device, trl_trainer** trainers_out, 
         std::vector<double> sets(tb->size() / 8);
         std::memcpy(sets.data(), tb->data(), tb->size());
         if (trl_set_terrain_slot(h, s, m.terrain_type[s], std::move(sets))) return bail("");
+    }
+    if (const auto* lb = need("phys_loaded", 0)) {
+        const auto* tb = need("phys_table", sizeof(PhysParams) * kMaxPhysSlots);
+        int32_t mask = 0;
+        if (lb->size() == 4) std::memcpy(&mask, lb->data(), 4);
+        if (!tb || lb->size() != 4 || mask == 0 || (mask & ~0xfe)) return bail("physics slots: table or slot mask missing or malformed");
+        PhysParams table[kMaxPhysSlots];
+        std::memcpy(table, tb->data(), sizeof(table));
+        for (int s = 1; s < kMaxPhysSlots; ++s) {
+            if (!(mask & (1 << s))) continue;
+            const PhysParams& q = table[s];
+            const double p7[7] = {q.kn, q.dn, q.mu, q.v_eps, q.contact_tol, q.k_lim, q.d_lim};
+            if (trl_load_physics(h, s, p7, q.vertex_contacts)) return bail("");
+        }
     }
     if ((m.policies || m.trainers) && !h->mc.has_net) return bail("the scene has no policy net");
     for (int p = 1; p < kMaxPolicySlots; ++p)

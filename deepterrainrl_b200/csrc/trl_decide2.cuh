@@ -290,6 +290,34 @@ __global__ void __launch_bounds__(1024) trl_cell_stats_kernel(Buffers B, const i
         }
 }
 
+// the same four figures over the envs of one (policy slot, terrain slot, physics slot) cell into out[4], -1 = any slot; one CTA with
+// trl_stats_kernel's traversal and reduction order.  The physics slot is the one of the env's present episode (env_phys row 0)
+__global__ void __launch_bounds__(1024) trl_phys_stats_kernel(Buffers B, const int* __restrict__ env_slot, const int* __restrict__ env_phys, int p,
+                                                              int t, int q, double* __restrict__ out) {
+    __shared__ double red[4][32];
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
+    const int* terrain_slot = B.i + (size_t)I_TERRAIN_SLOT * B.n;
+    double c = 0, e = 0, st = 0, ds = 0;
+    for (int env = threadIdx.x; env < B.n; env += blockDim.x) {
+        if (p >= 0 && (env_slot ? env_slot[env] : 0) != p) continue;
+        if (t >= 0 && terrain_slot[env] != t) continue;
+        if (q >= 0 && env_phys[env] != q) continue;
+        const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
+        c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
+        e += ec;
+        st += (double)(((uint64_t)(uint32_t)B.i[(size_t)I_STEPS_HI * B.n + env] << 32) | (uint32_t)B.i[(size_t)I_STEPS_LO * B.n + env]);
+        ds += B.d[(size_t)D_AVG_DIST * B.n + env] * ec;
+    }
+    c = warp_sum_all(c); e = warp_sum_all(e); st = warp_sum_all(st); ds = warp_sum_all(ds);
+    if (l == 0) { red[0][w] = c; red[1][w] = e; red[2][w] = st; red[3][w] = ds; }
+    __syncthreads();
+    if (w == 0)
+        for (int k = 0; k < 4; ++k) {
+            const double v = warp_sum_all(l < nw ? red[k][l] : 0.0);
+            if (l == 0) out[k] = v;
+        }
+}
+
 // the conv stage over the rows of a trainer minibatch (one cluster per row)
 __global__ void __cluster_dims__(kClusterSize, 1, 1) __launch_bounds__(kDecideThreads, 2)
 trl_fwd_conv_train_kernel(NetWeights W, FwdTrain f, double* __restrict__ act2) {
@@ -709,6 +737,10 @@ void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSetti
 }
 void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st) {
     TRL_LAUNCH(trl_cell_stats_kernel, (kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1), 1024, 0, st, B, env_slot, out);
+}
+void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot, double* out,
+                       cudaStream_t st) {
+    TRL_LAUNCH(trl_phys_stats_kernel, 1, 1024, 0, st, B, env_slot, env_phys, policy_slot, terrain_slot, phys_slot, out);
 }
 
 // the forward pass of a trainer minibatch through the same two kernels (trl_train.cu: enqueue_forward); act2 = [rows][5984] scratch the

@@ -72,6 +72,14 @@ struct trl_handle {
     bool terrain_loaded[trl::kMaxTerrainSlots] = {};           // [0] unused
     std::vector<int> env_terrain_host;                         // the assignment of every env (I_TERRAIN_SLOT_NEXT)
     double* cell_stats = nullptr;                              // [kMaxPolicySlots + 1][kMaxTerrainSlots + 1][4] (trl_eval_stats_cell)
+    // physics slots (trl_load_physics, any mode): slot 0 is mc.phys (trl_set_phys_params), copied into phys[0] at every upload; slots 1..
+    // hold loaded values.  phys[] is the __constant__ table of the physics-slot build.  Until a slot >= 1 is loaded env_phys is null,
+    // env_phys_host empty, every env on slot 0, and the step launches run the other builds
+    trl::PhysParams phys[trl::kMaxPhysSlots] = {};
+    bool phys_loaded[trl::kMaxPhysSlots] = {};                 // [0] unused
+    std::vector<int> env_phys_host;                            // the assignment of every env (row 1 of env_phys)
+    int* env_phys = nullptr;                                   // device [2][n]: slot of the present episode, slot from the next reset on
+    double* phys_stats = nullptr;                              // [4] (trl_eval_stats_phys)
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
     bool use_graph = true;

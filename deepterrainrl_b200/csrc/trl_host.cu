@@ -36,6 +36,8 @@ void launch_decide2(const Buffers& B, const NetWeights& W, const ExpSettings* ex
 void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSettings* ex, const FcMaps& maps, const FcSlotMaps& smaps, double* act2,
                           int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part);
 void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
+void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot, double* out,
+                       cudaStream_t st);
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
@@ -43,10 +45,19 @@ cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terr
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_cg
-// the terrain-slot builds of the env-step kernels (trl_step_ts.cu, trl_step_ts_cg.cu); the emulator's trl / trl_cg builds are those
+// the terrain-slot builds of the env-step kernels (trl_step_ts.cu, trl_step_ts_cg.cu) and the physics-slot builds (trl_step_ps.cu,
+// trl_step_ps_cg.cu); the emulator's trl / trl_cg builds are all of those
 #ifdef TRL_SIMT_EMU
+namespace trl {
+cudaError_t upload_phys(const PhysParams* phys, int* env_phys);
+}
+namespace trl_cg {
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+}
 namespace trl_ts = trl;
 namespace trl_ts_cg = trl_cg;
+namespace trl_ps = trl;
+namespace trl_ps_cg = trl_cg;
 #else
 namespace trl_ts {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
@@ -60,6 +71,20 @@ cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terr
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_ts_cg
+namespace trl_ps {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+void launch_reset(const trl::Buffers& B, const uint64_t* seeds, const int* env_ids, int count, int reseed, cudaStream_t st);
+void launch_terrain(const trl::Buffers& B, double lookahead, cudaStream_t st);
+}  // namespace trl_ps
+namespace trl_ps_cg {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+}  // namespace trl_ps_cg
 #endif
 
 
@@ -69,11 +94,15 @@ using namespace trl;
 struct trl_handle;
 static const trl_handle* g_model_owner = nullptr;    // whose ModelConst currently sits in the __constant__ copies
 static int g_device = -1;                             // the one device this process drives (set by the first handle)
-static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain) {
+static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys) {
     cudaError_t e = trl::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ts::upload_model(mc, terrain);
-    return e != cudaSuccess ? e : trl_ts_cg::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_ts_cg::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_ps::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_ps_cg::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_ps::upload_phys(phys, env_phys);
+    return e != cudaSuccess ? e : trl_ps_cg::upload_phys(phys, env_phys);
 }
 
 static thread_local std::string g_err;
@@ -107,7 +136,8 @@ static int ensure_model_only(trl_handle* h) {
     if (cudaDeviceSynchronize() != cudaSuccess) return 1;
     h->terrain[0].type = h->mc.terrain_type;      // slot 0 of the terrain table is the scene's own terrain
     std::memcpy(h->terrain[0].params, h->mc.terrain_params, sizeof(h->mc.terrain_params));
-    if (upload_model_all(h->mc, h->terrain) != cudaSuccess) return 1;
+    h->phys[0] = h->mc.phys;                      // and slot 0 of the physics table its own physics
+    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys) != cudaSuccess) return 1;
     g_model_owner = h;
     return 0;
 }
@@ -498,22 +528,28 @@ static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, 
     else if (part & 1)
         launch_decide(h->B, h->W, h->d_ex, h->done_count, h->decide_grid, list, rearm, st);
 }
-// the env-step launches of a handle: the terrain-slot builds once a terrain slot is loaded (trl_load_terrain), else the plain ones
+// the env-step launches of a handle: the physics-slot builds once a physics slot is loaded (trl_load_physics; they serve terrain
+// slots too), else the terrain-slot builds once a terrain slot is loaded (trl_load_terrain), else the plain ones
 static bool terrain_slots(const trl_handle* h) { return !h->env_terrain_host.empty(); }
+static bool phys_slots(const trl_handle* h) { return h->env_phys != nullptr; }
 static void step_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1) {
-    if (terrain_slots(h)) trl_ts::launch_step(h->B, step, flags, lists, st, group, n_groups);
+    if (phys_slots(h)) trl_ps::launch_step(h->B, step, flags, lists, st, group, n_groups);
+    else if (terrain_slots(h)) trl_ts::launch_step(h->B, step, flags, lists, st, group, n_groups);
     else launch_step(h->B, step, flags, lists, st, group, n_groups);
 }
 static void catchup_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st) {
-    if (terrain_slots(h)) trl_ts_cg::launch_step(h->B, step, flags, lists, st);
+    if (phys_slots(h)) trl_ps_cg::launch_step(h->B, step, flags, lists, st);
+    else if (terrain_slots(h)) trl_ts_cg::launch_step(h->B, step, flags, lists, st);
     else trl_cg::launch_step(h->B, step, flags, lists, st);
 }
 static void terrain_launch(const trl_handle* h, cudaStream_t st) {
-    if (terrain_slots(h)) trl_ts::launch_terrain(h->B, 0.5, st);
+    if (phys_slots(h)) trl_ps::launch_terrain(h->B, 0.5, st);
+    else if (terrain_slots(h)) trl_ts::launch_terrain(h->B, 0.5, st);
     else launch_terrain(h->B, 0.5, st);
 }
 static void reset_launch(const trl_handle* h, const uint64_t* seeds, const int* env_ids, int count, int reseed) {
-    if (terrain_slots(h)) trl_ts::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+    if (phys_slots(h)) trl_ps::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+    else if (terrain_slots(h)) trl_ts::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
     else launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
 }
 static int num_decide_launches(const trl_handle* h) { return h->decide_v2 ? (h->slots_active ? 3 : 2) : 1; }
@@ -723,7 +759,8 @@ trl_handle* trl_create_common(trl_handle* h, int num_envs, int device, int mode,
     g_model_owner = nullptr;
     if (ensure_model(h)) return bail("upload_model failed");
     if (!ck(configure_step_kernels(), "configure_step_kernels") || !ck(trl_cg::configure_step_kernels(), "configure_step_kernels") ||
-        !ck(trl_ts::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ts_cg::configure_step_kernels(), "configure_step_kernels"))
+        !ck(trl_ts::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ts_cg::configure_step_kernels(), "configure_step_kernels") ||
+        !ck(trl_ps::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ps_cg::configure_step_kernels(), "configure_step_kernels"))
         return bail("");
     if (!ck(configure_decide_kernel(), "configure_decide_kernel")) return bail("");
     if (!ck(configure_decide2_kernels(), "configure_decide2_kernels")) return bail("");
@@ -1443,6 +1480,100 @@ int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episo
     if (!h) return fail("trl_eval_stats_slot: null handle");
     if (slot < 0 || slot >= kMaxPolicySlots) return fail("trl_eval_stats_slot: slot " + std::to_string(slot) + " out of range");
     return eval_stats_cell(h, "trl_eval_stats_slot", slot, -1, cycles, episodes, avg_dist, env_steps);
+}
+
+static bool phys_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxPhysSlots && h->phys_loaded[slot]); }
+
+int trl_load_physics(trl_handle* h, int slot, const double* p, int vertex_contacts) {
+    const std::string who = "trl_load_physics";
+    if (!h) return fail(who + ": null handle");
+    if (slot < 1 || slot >= kMaxPhysSlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxPhysSlots - 1) + "; slot 0 is the scene's physics, set by trl_set_phys_params)");
+    if (!p) return fail(who + ": null parameter array");
+    static const char* names[7] = {"kn", "dn", "mu", "v_eps", "contact_tol", "k_lim", "d_lim"};
+    for (int k = 0; k < 7; ++k)
+        if (!std::isfinite(p[k])) return fail(who + ": " + names[k] + " is not finite");
+    for (int k : {0, 1, 2, 5, 6})
+        if (p[k] < 0.0) return fail(who + ": " + names[k] + " = " + std::to_string(p[k]) + " is negative");
+    if (!(p[3] > 0.0)) return fail(who + ": v_eps = " + std::to_string(p[3]) + " must be positive");
+    if (p[4] * std::sqrt(1.0 + kMaxSlope * kMaxSlope) > kClearMargin)
+        return fail(who + ": contact_tol = " + std::to_string(p[4]) + " exceeds what the broad phase covers (contact_tol * sqrt(1 + 25^2) <= 0.05)");
+    if (drain(h)) return 1;
+    if (!h->env_phys) {     // first slot: from now on the step launches run the physics-slot build
+        int* d = nullptr;
+        CK(dalloc(h, &d, 2 * (size_t)h->n));
+        h->env_phys = d;
+        h->env_phys_host.assign((size_t)h->n, 0);
+        destroy_graphs(h);
+    }
+    h->phys[slot] = PhysParams{p[0], p[1], p[2], p[3], p[4], p[5], p[6], vertex_contacts ? 1 : 0};
+    h->phys_loaded[slot] = true;
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail(who + ": physics table upload failed") : 0;
+}
+
+int trl_set_env_physics(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
+    const std::string who = "trl_set_env_physics";
+    if (!h) return fail(who + ": null handle");
+    if (n < 0 || n > h->n) return fail(who + ": env count out of range");
+    if (n > 0 && !slots) return fail(who + ": null slot list");
+    for (int k = 0; k < n; ++k) {
+        const int e = env_ids ? env_ids[k] : k;
+        if (e < 0 || e >= h->n) return fail(who + ": env id " + std::to_string(e) + " out of range");
+        if (slots[k] < 0 || slots[k] >= kMaxPhysSlots) return fail(who + ": slot " + std::to_string(slots[k]) + " out of range");
+        if (!phys_loaded(h, slots[k])) return fail(who + ": slot " + std::to_string(slots[k]) + " is empty (trl_load_physics first)");
+    }
+    if (!h->env_phys) return 0;      // only slot 0 exists, and every env is on it
+    std::vector<int> next = h->env_phys_host;
+    for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = slots[k];
+    if (drain(h)) return 1;
+    CK(cudaMemcpy(h->env_phys + h->n, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
+    h->env_phys_host.swap(next);
+    return 0;
+}
+
+int trl_env_physics(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
+    if (!h) return fail("trl_env_physics: null handle");
+    if (n < 0 || n > h->n) return fail("trl_env_physics: env count out of range");
+    if (!h->env_phys) {
+        for (int k = 0; k < n; ++k) {
+            if (current) current[k] = 0;
+            if (assigned) assigned[k] = 0;
+        }
+        return 0;
+    }
+    if (drain(h)) return 1;
+    if (current && n > 0) CK(cudaMemcpy(current, h->env_phys, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (assigned && n > 0) CK(cudaMemcpy(assigned, h->env_phys + h->n, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+// a cell with any physics slot, or any cell of a handle whose envs are all on physics slot 0, is trl_eval_stats_cell's; the others come
+// from trl_phys_stats_kernel
+int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes, double* avg_dist,
+                        int64_t* env_steps) {
+    const std::string who = "trl_eval_stats_phys";
+    if (!h) return fail(who + ": null handle");
+    if (phys_slot < -1 || phys_slot >= kMaxPhysSlots) return fail(who + ": physics slot " + std::to_string(phys_slot) + " out of range");
+    if (phys_slot >= 0 && !phys_loaded(h, phys_slot)) return fail(who + ": physics slot " + std::to_string(phys_slot) + " is empty");
+    if (phys_slot < 0 || !h->env_phys) return eval_stats_cell(h, who.c_str(), policy_slot, terrain_slot, cycles, episodes, avg_dist, env_steps);
+    if (policy_slot < -1 || policy_slot >= kMaxPolicySlots) return fail(who + ": policy slot " + std::to_string(policy_slot) + " out of range");
+    if (policy_slot >= 0 && !slot_loaded(h, policy_slot)) return fail(who + ": policy slot " + std::to_string(policy_slot) + " is empty");
+    if (terrain_slot < -1 || terrain_slot >= kMaxTerrainSlots) return fail(who + ": terrain slot " + std::to_string(terrain_slot) + " out of range");
+    if (terrain_slot >= 0 && !terrain_loaded(h, terrain_slot)) return fail(who + ": terrain slot " + std::to_string(terrain_slot) + " is empty");
+    if (!h->phys_stats) CK(dalloc(h, &h->phys_stats, 4));
+    double st[4];
+    launch_phys_stats(h->B, h->slots_active ? h->P.env_slot : nullptr, h->env_phys, h->slots_active ? policy_slot : -1,
+                      h->env_terrain_host.empty() ? -1 : terrain_slot, phys_slot, h->phys_stats, h->stream);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(st, h->phys_stats, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (cycles) *cycles = (int64_t)st[0];
+    if (episodes) *episodes = (int64_t)st[1];
+    if (env_steps) *env_steps = (int64_t)st[2];
+    if (avg_dist) *avg_dist = st[1] > 0 ? st[3] / st[1] : 0.0;
+    return 0;
 }
 
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {

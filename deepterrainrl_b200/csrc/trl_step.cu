@@ -41,7 +41,14 @@
 // compiled with TRL_TERRAIN_SLOTS_VARIANT: their envs generate their ground from their own slot of c_terrain.  The builds without it
 // generate from c_model's terrain, so a handle without terrain slots runs the same kernels as before slots existed.  The emulator
 // (tests/simt) compiles only trl_step.cu / trl_step_cg.cu and always with slots, which computes the same for a handle without any.
-#if defined(TRL_TERRAIN_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
+// Physics slots (trl_load_physics) are served by a third pair, trl_step_ps.cu (namespace trl_ps) and trl_step_ps_cg.cu (trl_ps_cg),
+// compiled with TRL_PHYS_SLOTS_VARIANT as well as TRL_TERRAIN_SLOTS_VARIANT: their physics sub-steps read the env's own slot of
+// c_phys.  The emulator's "always with slots" includes physics slots; a handle without any has no per-env array and reads slot 0.
+#if defined(TRL_PHYS_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
+#define TRL_IMPL_NS trl_ps_cg
+#elif defined(TRL_PHYS_SLOTS_VARIANT)
+#define TRL_IMPL_NS trl_ps
+#elif defined(TRL_TERRAIN_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
 #define TRL_IMPL_NS trl_ts_cg
 #elif defined(TRL_TERRAIN_SLOTS_VARIANT)
 #define TRL_IMPL_NS trl_ts
@@ -61,6 +68,14 @@ constexpr bool kTerrainSlots = false;
 
 __constant__ ModelConst c_model;
 __constant__ TerrainSlot c_terrain[kMaxTerrainSlots];    // slot 0 = c_model's terrain_type / terrain_params (trl_types.h: TerrainSlot)
+#if defined(TRL_PHYS_SLOTS_VARIANT) || defined(TRL_SIMT_EMU)
+#define TRL_PHYS_TABLE 1
+__constant__ PhysParams c_phys[kMaxPhysSlots];   // slot 0 = c_model.phys (trl_types.h: kMaxPhysSlots)
+__constant__ int* c_env_phys;                    // [2][n] of the owning handle: the physics slot of every env's present episode, then
+                                                 // the slot it gets at its next reset; null while the handle has no physics slot
+#else
+#define TRL_PHYS_TABLE 0
+#endif
 // character-type branches: a run-time constant of the scene (the raptor's controller differs from the dog's / goat's); an experiment
 // build can fix it at compile time (-DTRL_FIXED_CHAR=0 dog / goat, 2 raptor) to see what the unused branches cost
 #ifdef TRL_FIXED_CHAR
@@ -95,7 +110,6 @@ constexpr unsigned kFull = 0xffffffffu;
 constexpr int kStepSkipPending = 8, kStepCatchUp = 16;   // flag bits of trl_step_kernel beyond ctrl (1) / phys (2) / end (4)
 // `lists` packs: bits 0-2 the list new boundary envs are appended to, bits 3-5 the list a catch-up launch serves, bits 6-9 the number
 // of env-steps a catch-up launch advances its envs by
-constexpr double kClearMargin = 0.05;   // >= contact_tol * sqrt(1 + slope^2) for any slope the generators produce
 constexpr int kZeroLane = 31;   // always idle (nj <= 23): its per-link registers are zero, used as the "no source" lane
 // per-warp shared scratch (doubles; every block starts 16-byte aligned)
 // Link block: one slot per link, written by the link lanes and walked by the chain lanes (chain_inward / chain_outward).  A slot is
@@ -188,6 +202,14 @@ __device__ unsigned long long g_phase_clocks[kNumPhases + 1];
 #define TRL_REUSE_KIN_DECL , const Kin* k0
 #else
 #define TRL_REUSE_KIN_DECL
+#endif
+// the physics slot of the env a sub-step serves (physics-slot builds only: the other builds keep the parent's signature)
+#if TRL_PHYS_TABLE
+#define TRL_PS_DECL , int ps
+#define TRL_PS_ARG , ps
+#else
+#define TRL_PS_DECL
+#define TRL_PS_ARG
 #endif
 
 // 128-bit shared-memory accesses of the experiment builds need 16-byte aligned addresses (a misaligned one faults on the GPU);
@@ -1029,13 +1051,18 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
 // One sub-step of articulated-body forward dynamics with linearly-implicit contact / joint-limit terms.
 // Updates e (q, qd, root translation) in place and returns the contact bitmask (same value in every lane).
 __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g, const double* s_clx, const double* s_cly,
-                               int lane, double dt, double clear_y, double* xs TRL_REUSE_KIN_DECL) {
+                               int lane, double dt, double clear_y, double* xs TRL_REUSE_KIN_DECL TRL_PS_DECL) {
     const double lk_mass = lc.mass;      // read once (shared-memory table; a read cannot move across the shuffles below)
     // per-body box tables (link frame): centre offset, axis rotation, half sizes -- staged by the kernel next to the corner tables
     const double *s_bax = s_clx + 4 * kMaxJoints, *s_bay = s_bax + kMaxJoints, *s_bc = s_bay + kMaxJoints, *s_bs = s_bc + kMaxJoints,
                  *s_hx = s_bs + kMaxJoints, *s_hy = s_hx + kMaxJoints;
     const ModelConst& m = c_model;
+#if TRL_PHYS_TABLE
+    // the env's slot: ps is the same in every lane (one env per warp), so each read is one broadcast from the constant cache
+    const PhysParams& pp = c_phys[ps];
+#else
     const PhysParams& pp = m.phys;
+#endif
     TRL_CLK_BEGIN(clk);
 #if TRL_REUSE_KIN
     Kin k;
@@ -1156,7 +1183,13 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
     // one-sided implicit spring-damper at the joint limits (branch-free: the range of a free joint is infinite)
     const double viol = fmax(e.q - lc.lim_hi, 0.0) + fmin(e.q - lc.lim_lo, 0.0);
     const double cl = (viol != 0.0) ? pp.d_lim + dt * pp.k_lim : 0.0;
+#if TRL_PHYS_TABLE
+    // the FMA the builds reading c_model.phys make of k_lim * viol + cl * qd, spelled out: with the parameters in a register-indexed
+    // table the compiler fuses the other product, which rounds differently
+    const double lim_f = __fma_rn(viol, pp.k_lim, cl * e.qd);
+#else
     const double lim_f = pp.k_lim * viol + cl * e.qd;
+#endif
     double* slot = xs + X_LNK + lane * kLinkStride;
     if (lc.act) {
         store_vals(slot, ia);
@@ -1249,6 +1282,9 @@ __device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B
             slot = L.I[(size_t)I_TERRAIN_SLOT_NEXT * L.n + L.env];
             L.I[(size_t)I_TERRAIN_SLOT * L.n + L.env] = slot;
         }
+#if TRL_PHYS_TABLE
+        if (c_env_phys) c_env_phys[L.env] = c_env_phys[(size_t)L.n + L.env];   // likewise the physics slot (trl_set_env_physics)
+#endif
         GroundView g = load_ground(L, B);
         g.n[0] = g.n[1] = 0; g.flip = 0;
         if constexpr (kTerrainSlots) g.update(-11.0, 9.0, c_terrain[slot].type, c_terrain[slot].params, 20.0);
@@ -1470,11 +1506,15 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         // terrain maximum over the window the character's corners can reach during this env-step; kClearMargin covers the
         // contact tolerance measured along the surface normal on (near-)vertical cliff faces and the root's travel
         const double clear_y = g.window_max(e.ox - m.reach - 0.25, e.ox + m.reach + 0.25, lane) + kClearMargin;
+#if TRL_PHYS_TABLE
+        // the slot of the env's present episode (a reset above has already made its assignment current)
+        const int ps = c_env_phys ? c_env_phys[env] : 0;
+#endif
 #if TRL_REUSE_KIN
         for (int s = 0; s < ns; ++s)
-            contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs, (s == 0 && have_k) ? &k_ctrl : nullptr);
+            contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs, (s == 0 && have_k) ? &k_ctrl : nullptr TRL_PS_ARG);
 #else
-        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs);
+        for (int s = 0; s < ns; ++s) contact = physics_substep(lc, e, g, s_clx, s_cly, lane, dt, clear_y, xs TRL_PS_ARG);
 #endif
         TRL_CLK_RESET(clk);
         // UpdateGround (scenarios/ScenarioSimChar.cpp:564-572): regenerate a segment when the view window crosses it
@@ -1657,6 +1697,14 @@ cudaError_t upload_model(const ModelConst& mc, const TerrainSlot* terrain) {
 #endif
     return e;
 }
+#if TRL_PHYS_TABLE
+// the physics table (slot 0 = mc.phys) and the handle's per-env slot array (null: every env on slot 0), uploaded with the model
+cudaError_t upload_phys(const PhysParams* phys, int* env_phys) {
+    cudaError_t e = cudaMemcpyToSymbol(c_phys, phys, sizeof(PhysParams) * kMaxPhysSlots);
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_phys, &env_phys, sizeof(env_phys));
+    return e;
+}
+#endif
 size_t step_smem_bytes() { return 0; }
 // TRL_PHASE_CLOCKS builds: copy the accumulated phase clocks (kNumPhases + the env-step count) into out[], optionally zero them
 cudaError_t step_phase_clocks(unsigned long long* out, int reset) {
@@ -1704,7 +1752,7 @@ void launch_reset(const Buffers& B, const uint64_t* seeds, const int* env_ids, i
 
 }  // namespace TRL_IMPL_NS
 
-#if !defined(TRL_CG_VARIANT) && !defined(TRL_TERRAIN_SLOTS_VARIANT)
+#if !defined(TRL_CG_VARIANT) && !defined(TRL_TERRAIN_SLOTS_VARIANT) && !defined(TRL_PHYS_SLOTS_VARIANT)
 #include "trl_decide.cuh"
 #include "trl_decide2.cuh"
 #endif

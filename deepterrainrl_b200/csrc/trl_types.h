@@ -157,6 +157,18 @@ struct TerrainSlot {
     double params[kTerrainParams];
 };
 
+// Physics slots: slot 0 is the scene's own PhysParams (ModelConst::phys), slots 1 .. kMaxPhysSlots - 1 are loaded by
+// trl_load_physics.  The table sits in __constant__ memory of the physics-slot build beside the model and is uploaded with it; the
+// per-env slots ([2][n]: current, assigned) are an allocation of their own, so ModelConst, Buffers and the planes keep their layout.
+constexpr int kMaxPhysSlots = 8;
+// Broad phase of the env-step: a box corner more than kClearMargin above the terrain maximum under the character is no contact
+// candidate.  That holds while contact_tol * sqrt(1 + slope^2) <= kClearMargin for every slope the corner can meet.  The steepest
+// slope of the generators with the shipped terrain files and defaults is a 2 m gap wall between two vertices 0.1 m apart, plus the
+// slope overlay and bumps: below kMaxSlope.  trl_load_physics refuses a contact tolerance above kClearMargin / sqrt(1 + kMaxSlope^2)
+// (0.001998 m; the scenes' own is 0.00025 m).
+constexpr double kClearMargin = 0.05;
+constexpr double kMaxSlope = 25.0;
+
 // Exploration settings can change between updates (cScenarioExp::SetExpRate/Temp/BaseActionRate).
 struct ExpSettings {
     int enable;

@@ -46,7 +46,7 @@ VARIANTS = {
     "smem_xchg_decide_tile4": ["-DTRL_SMEM_XCHG=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
     "all": ["-DTRL_SMEM_XCHG=1", "-DTRL_REUSE_KIN=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
 }
-STEP_UNITS = ("trl_step.cu", "trl_step_cg.cu", "trl_step_ts.cu", "trl_step_ts_cg.cu")      # the only translation units the variant flags reach
+STEP_UNITS = ("trl_step.cu", "trl_step_cg.cu", "trl_step_ts.cu", "trl_step_ts_cg.cu", "trl_step_ps.cu", "trl_step_ps_cg.cu")      # the only translation units the variant flags reach
 
 
 def _variant():
@@ -71,7 +71,8 @@ def library_path():
 def build_library(force=False, verbose=False):
     """Compile csrc/*.cu for sm_90a into lib/libterrainrl_b200.so (nvcc cross-compiles without a GPU).
     trl_step_cg.cu is the env-step translation unit again with -Xptxas -dlcm=cg (L1-bypassing loads, see trl_step.cu);
-    trl_step_ts.cu / trl_step_ts_cg.cu are both again with terrain slots.
+    trl_step_ts.cu / trl_step_ts_cg.cu are both again with terrain slots, trl_step_ps.cu / trl_step_ps_cg.cu with terrain and
+    physics slots.
     With TRL_VARIANT set, the two env-step units are compiled with the variant's flags and linked with the product's other
     objects into lib/variants/<name>/."""
     variant = _variant()
@@ -84,6 +85,7 @@ def build_library(force=False, verbose=False):
     out = library_path()
     csrc = os.path.join(_PKG, "csrc")
     units = [("trl_step.cu", []), ("trl_step_cg.cu", ["-Xptxas", "-dlcm=cg"]), ("trl_step_ts.cu", []), ("trl_step_ts_cg.cu", ["-Xptxas", "-dlcm=cg"]),
+             ("trl_step_ps.cu", []), ("trl_step_ps_cg.cu", ["-Xptxas", "-dlcm=cg"]),
              ("trl_host.cu", []), ("trl_train.cu", []), ("trl_checkpoint.cu", []),
              ("trl_comm.cu", []), ("trl_probe.cu", []), ("trl_tc_policy.cu", []), ("ref_loader.cpp", [])]
     deps = [os.path.join(csrc, f) for f in os.listdir(csrc)]
@@ -134,6 +136,7 @@ EXPORTS = [
     "trl_trainer_create_slot", "trl_train_run_slots", "trl_output_model_slot",
     "trl_set_explore_slot", "trl_train_run_slots_sched",
     "trl_checkpoint_save", "trl_create_from_checkpoint", "trl_trainer_params", "trl_env_policy",
+    "trl_load_physics", "trl_set_env_physics", "trl_env_physics", "trl_eval_stats_phys",
 ]
 
 
@@ -283,6 +286,29 @@ class BatchedScenario:
         cur = np.zeros(self.num_envs, np.int32)
         nxt = np.zeros(self.num_envs, np.int32)
         self._ck(self.L.trl_env_terrain(self.h, _p(cur), _p(nxt), self.num_envs))
+        return cur, nxt
+
+    def LoadPhysics(self, slot, p7, vertex_contacts=False):
+        """contact / joint-limit parameters (SetPhysParams order: kn, dn, mu, v_eps, contact_tol, k_lim, d_lim) and the vertex contact
+        model into physics slot 1..7; envs move to it with SetEnvPhysics.  Reloading a slot acts from the next env-step."""
+        a = np.ascontiguousarray(p7, dtype=np.float64).ravel()
+        if a.size != 7:
+            raise ValueError("LoadPhysics: 7 parameters")
+        self._ck(self.L.trl_load_physics(self.h, int(slot), _p(a), int(bool(vertex_contacts))))
+
+    def SetEnvPhysics(self, slots, env_ids=None):
+        """env_ids[k] (default: env k) runs on physics slot slots[k] from its next episode reset on"""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        if ids is not None and ids.size != s.size:
+            raise ValueError("SetEnvPhysics: one slot per env id")
+        self._ck(self.L.trl_set_env_physics(self.h, _p(ids), _p(s), int(s.size)))
+
+    def EnvPhysics(self):
+        """(current, assigned): per env, the physics slot of its present episode and the one it gets at its next reset"""
+        cur = np.zeros(self.num_envs, np.int32)
+        nxt = np.zeros(self.num_envs, np.int32)
+        self._ck(self.L.trl_env_physics(self.h, _p(cur), _p(nxt), self.num_envs))
         return cur, nxt
 
     def GetOutputOffsetScale(self):
@@ -435,11 +461,14 @@ class BatchedScenario:
     def GetNumEnvSteps(self):
         return self._stats()["steps"]
 
-    def GetEvalStats(self, slot=0, terrain=None):
+    def GetEvalStats(self, slot=0, terrain=None, physics=None):
         """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot` (None: any) whose present ground comes from
-        terrain slot `terrain` (None: any)"""
+        terrain slot `terrain` (None: any) and whose present episode runs on physics slot `physics` (None: any)"""
         c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
-        if terrain is None and slot is not None:
+        if physics is not None:
+            rc = self.L.trl_eval_stats_phys(self.h, -1 if slot is None else int(slot), -1 if terrain is None else int(terrain), int(physics),
+                                            C.byref(c), C.byref(e), C.byref(a), C.byref(s))
+        elif terrain is None and slot is not None:
             rc = self.L.trl_eval_stats_slot(self.h, int(slot), C.byref(c), C.byref(e), C.byref(a), C.byref(s))
         else:
             rc = self.L.trl_eval_stats_cell(self.h, -1 if slot is None else int(slot), -1 if terrain is None else int(terrain),
@@ -447,9 +476,9 @@ class BatchedScenario:
         self._ck(rc)
         return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
 
-    def GetDistLog(self, slot=None, terrain=None):
-        """(distances, env ids) of the episodes logged so far; slot / terrain: only the entries of envs now on that policy slot / whose
-        present ground comes from that terrain slot"""
+    def GetDistLog(self, slot=None, terrain=None, physics=None):
+        """(distances, env ids) of the episodes logged so far; slot / terrain / physics: only the entries of envs now on that policy slot
+        / whose present ground comes from that terrain slot / whose present episode runs on that physics slot"""
         d = C.c_void_p(); e = C.c_void_p(); n = C.c_int(0)
         self._ck(self.L.trl_dist_log(self.h, C.byref(d), C.byref(e), C.byref(n)))
         if n.value == 0:
@@ -461,6 +490,9 @@ class BatchedScenario:
             dist, env = dist[keep], env[keep]
         if terrain is not None:
             keep = self.EnvTerrain()[0][env] == terrain
+            dist, env = dist[keep], env[keep]
+        if physics is not None:
+            keep = self.EnvPhysics()[0][env] == physics
             dist, env = dist[keep], env[keep]
         return dist, env
 

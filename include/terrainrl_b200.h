@@ -203,6 +203,28 @@ int trl_set_env_terrain(trl_handle* h, const int32_t* env_ids, const int32_t* sl
 int trl_env_terrain(trl_handle* h, int32_t* current, int32_t* assigned, int n);
 int trl_eval_stats_cell(trl_handle* h, int policy_slot, int terrain_slot, int64_t* cycles, int64_t* episodes, double* avg_dist,
                         int64_t* env_steps);
+/* Physics slots (any mode, with or without trainers, policy or terrain slots): up to 8 contact / joint-limit settings per handle.
+ * Slot 0 is the handle's own, which trl_set_phys_params edits; slots 1..7 start empty.  With the same seeds, env i on physics slot q
+ * computes bit for bit what env i computes in a handle whose trl_set_phys_params holds slot q's values (created with
+ * TRL_VERTEX_CONTACTS=1 when the slot has vertex contacts).
+ *   trl_load_physics      p7 (trl_set_phys_params order: kn, dn, mu, v_eps, contact_tol, k_lim, d_lim) and the vertex contact model
+ *                         (0 off, else on) into slot 1..7.  Refused, handle unchanged, for slot 0 or >= 8, a null p7, a non-finite
+ *                         value, kn, dn, mu, k_lim or d_lim < 0, v_eps <= 0, or contact_tol * sqrt(1 + 25^2) > 0.05, i.e.
+ *                         contact_tol > 0.001998: the broad phase keeps corners within 0.05 m of the terrain maximum, and 25 bounds
+ *                         the steepest slope the generators produce with the shipped terrain files (a 2 m gap wall over one 0.1 m
+ *                         vertex spacing, plus slopes and bumps).  Reloading a slot applies from the next env-step to every env on it,
+ *                         as trl_set_phys_params does for slot 0.
+ *   trl_set_env_physics   env_ids[k] (NULL: env k) -> slots[k] for k < n; every env starts on slot 0.  Refused, with nothing changed,
+ *                         for an env id or slot out of range, n > num_envs or an empty slot.  Takes effect at the env's next episode
+ *                         reset (a fall inside trl_update, trl_reset, trl_seed_terrain): an episode never mixes two settings.
+ *   trl_env_physics       per env (first n), the slot of its present episode and the slot it gets at its next reset.
+ *   trl_eval_stats_phys   trl_eval_stats_cell over the envs of one (policy, terrain, physics) cell, -1 = any slot; an env counts
+ *                         toward the physics slot of its present episode.  (p, t, -1) is trl_eval_stats_cell(p, t). */
+int trl_load_physics(trl_handle* h, int slot, const double* p7, int vertex_contacts);
+int trl_set_env_physics(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n);
+int trl_env_physics(trl_handle* h, int32_t* current, int32_t* assigned, int n);
+int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
+                        double* avg_dist, int64_t* env_steps);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
