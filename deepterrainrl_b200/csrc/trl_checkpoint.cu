@@ -190,6 +190,10 @@ int handle_state(trl_handle* h, std::vector<CkptSection>* out) {
         host("env_phys_host", 1, h->env_phys_host.data(), n * 4);
         fixed("env_phys", 1, h->env_phys, 2 * n * 4);
     }
+    if (h->env_eval) {       // evaluation envs: likewise written only once trl_set_env_eval has been called
+        host("env_eval_host", 1, h->env_eval_host.data(), n * 4);
+        fixed("env_eval", 1, h->env_eval, 2 * n * 4);
+    }
     fixed("B.d", 3, B.d, (size_t)D_NUM_FIELDS * n * 8);
     fixed("B.i", 1, B.i, (size_t)I_NUM_PLANES * n * 4);
     fixed("B.terrain", 2, B.terrain, n * 2 * kTerrainCap * 4);
@@ -290,6 +294,10 @@ int save_impl(trl_handle* h, const char* path, const void* user, size_t user_byt
         build.push_back(blob_of("phys_loaded", 1, &mask, 1));
         build.push_back(blob_of("phys_table", 0, h->phys, kMaxPhysSlots));
     }
+    if (h->env_eval) {
+        const int32_t on = 1;
+        build.push_back(blob_of("eval_envs", 1, &on, 1));
+    }
     build.insert(build.begin() + 1, blob_of("meta", 0, &m, 1));
     build.push_back(blob_of("user", 0, (const unsigned char*)user, user_bytes));
     std::vector<CkptSection> all;
@@ -389,8 +397,10 @@ trl_handle* load_impl(const char* path, int device, trl_trainer** trainers_out, 
     if (!mb || !sb || !ub) return refuse("the scene, meta or user section is missing or has the wrong size");
     Meta m;
     std::memcpy(&m, mb->data(), sizeof(m));
+    const auto* eb = need("eval_envs", 0);       // evaluation envs: the slot build runs even with slot 0 alone
+    if (eb && (eb->size() != 4 || m.mode != TRL_MODE_EXPLORE)) return refuse("the eval_envs section is malformed");
     if (m.n <= 0 || (m.mode != TRL_MODE_POLI_EVAL && m.mode != TRL_MODE_EXPLORE) || (m.trainers & ~0xff) || (m.policies & ~0xfe) ||
-        (m.terrains & ~0xfe) || (m.slots_active != 0) != ((m.policies | (m.trainers & 0xfe)) != 0))
+        (m.terrains & ~0xfe) || (m.slots_active != 0) != ((m.policies | (m.trainers & 0xfe)) != 0 || eb != nullptr))
         return refuse("inconsistent meta section");
     if (m.trainers && !trainers_out) return refuse("the checkpoint holds trainers: pass an array of 8 to receive them");
     auto* h = new trl_handle();
@@ -433,7 +443,8 @@ trl_handle* load_impl(const char* path, int device, trl_trainer** trainers_out, 
             if (trl_load_physics(h, s, p7, q.vertex_contacts)) return bail("");
         }
     }
-    if ((m.policies || m.trainers) && !h->mc.has_net) return bail("the scene has no policy net");
+    if ((m.policies || m.trainers || eb) && !h->mc.has_net) return bail("the scene has no policy net");
+    if (eb && trl_enable_env_eval(h)) return bail("");
     for (int p = 1; p < kMaxPolicySlots; ++p)
         if ((m.policies & (1 << p)) && trl_stage_slot_model(h, p, nullptr, nullptr)) return bail("");
     for (int p = 0; p < kMaxPolicySlots; ++p) {

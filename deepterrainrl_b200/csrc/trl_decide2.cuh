@@ -291,9 +291,10 @@ __global__ void __launch_bounds__(1024) trl_cell_stats_kernel(Buffers B, const i
 }
 
 // the same four figures over the envs of one (policy slot, terrain slot, physics slot) cell into out[4], -1 = any slot; one CTA with
-// trl_stats_kernel's traversal and reduction order.  The physics slot is the one of the env's present episode (env_phys row 0)
+// trl_stats_kernel's traversal and reduction order.  The physics slot is the one of the env's present episode (env_phys row 0).
+// env_eval (optional, null: any mode): only the envs whose present episode's mode (row 0 of trl_set_env_eval's array) is `eval`
 __global__ void __launch_bounds__(1024) trl_phys_stats_kernel(Buffers B, const int* __restrict__ env_slot, const int* __restrict__ env_phys, int p,
-                                                              int t, int q, double* __restrict__ out) {
+                                                              int t, int q, const int* __restrict__ env_eval, int eval, double* __restrict__ out) {
     __shared__ double red[4][32];
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
     const int* terrain_slot = B.i + (size_t)I_TERRAIN_SLOT * B.n;
@@ -302,6 +303,7 @@ __global__ void __launch_bounds__(1024) trl_phys_stats_kernel(Buffers B, const i
         if (p >= 0 && (env_slot ? env_slot[env] : 0) != p) continue;
         if (t >= 0 && terrain_slot[env] != t) continue;
         if (q >= 0 && env_phys[env] != q) continue;
+        if (env_eval && env_eval[env] != eval) continue;
         const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
         c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
         e += ec;
@@ -334,10 +336,13 @@ trl_fwd_conv_train_kernel(NetWeights W, FwdTrain f, double* __restrict__ act2) {
 // the scalar decision of one env (cDogControllerMACE::UpdateAction, cBaseControllerMACE::DecideActionBoltzmann, BuildActorAction,
 // ApplyExpNoiseAction: sim/DogController.cpp:847-868, sim/BaseControllerMACE.cpp:254-318,339-396,437-518); Y = this decision's
 // unnormalised net output (unused when the scene has no net).  kSlots: the exploration noise is scaled by the deciding slot's own actor
-// output scale `noise_scale` (the net of a training slot sets it); otherwise by the scene's, c_model.out_scale_actor0
+// output scale `noise_scale` (the net of a training slot sets it); otherwise by the scene's, c_model.out_scale_actor0.  An evaluating
+// env (kSlots only: trl_set_env_eval) decides with exploration off, whatever the settings `ex` of its slot say
 template <bool kSlots = false>
-__device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, const double* Y, const double* noise_scale = nullptr) {
+__device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, const double* Y, const double* noise_scale = nullptr,
+                           bool evaluates = false) {
     const ModelConst& m = c_model;
+    const bool slot_explores = kSlots && ex.enable && !evaluates;     // read where the single-policy build reads ex.enable
     Lane L{nullptr, env, B.n, B.d, B.i};
     double params[kNumParams];
     int id, eflags = 4;
@@ -351,7 +356,7 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
         L.i(I_CMD) = -1;
     } else if (m.has_net) {
         const double base_rand = rng.uniform();
-        if (ex.enable && base_rand < ex.base_rate) {
+        if ((kSlots ? slot_explores : ex.enable) && base_rand < ex.base_rate) {
             const int a = rng.rand_int(0, m.n_actions);
             id = build_base_action(L, rng, a, params);
             eflags = 4 | 3;
@@ -362,7 +367,7 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
             int a_max = 0;
             for (int i = 1; i < nf; ++i) if (Y[i] > Y[a_max]) a_max = i;
             int a = a_max;
-            if (ex.enable && ex.temp != 0.0) {   // BoltzmannSelectActor
+            if ((kSlots ? slot_explores : ex.enable) && ex.temp != 0.0) {   // BoltzmannSelectActor
                 double vals[8], sum = 0.0;
                 for (int i = 0; i < nf; ++i) { vals[i] = exp((Y[i] - Y[a_max]) / ex.temp); sum += vals[i]; }
                 double r = rng.uniform() * sum;
@@ -372,7 +377,7 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
             for (int k = 0; k < fs; ++k) params[m.opt_idx[k]] = Y[nf + a * fs + k];
             params[mTransTime] = fabs(params[mTransTime]); params[mCv] = fabs(params[mCv]);
             if (m.char_type == 2) params[rmCd] = fabs(params[rmCd]);
-            if (ex.enable) {
+            if (kSlots ? slot_explores : ex.enable) {
                 const double rn = rng.uniform();
                 if (rn < ex.rate) {              // ApplyExpNoiseAction
                     for (int k = 0; k < fs; ++k) params[m.opt_idx[k]] += (ex.noise * rng.normal()) * (1.0 / (kSlots ? noise_scale[k] : m.out_scale_actor0[k]));
@@ -396,7 +401,8 @@ __device__ void decide_one(const Buffers& B, const ExpSettings& ex, int env, con
 // cluster moves on to a chunk of another slot.  Without it, the single-policy kernel: chunk k = rows 32 k .., W0 = the one net.
 template <bool kTrain, bool kSlots = false>
 __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0, const ExpSettings* __restrict__ ex_dev, const FcMaps& maps, const FwdTrain& ft,
-                                         int* done_count, int list, int rearm, const FcSlotMaps* smaps = nullptr, const int* __restrict__ tab = nullptr) {
+                                         int* done_count, int list, int rearm, const FcSlotMaps* smaps = nullptr, const int* __restrict__ tab = nullptr,
+                                         const int* __restrict__ env_eval = nullptr) {
     TRL_DYN_SHARED(unsigned char, fc_smem_raw);
     // the swizzled TMA tiles need 1024-byte alignment; the dynamic window starts at the same offset in every CTA of the cluster, so
     // the rounded address is a valid DSMEM offset as well
@@ -667,7 +673,10 @@ __device__ __forceinline__ void fc_stage(const Buffers& B, const NetWeights& W0,
         }
         // ---------------- the scalar decisions of this chunk, one lane each
         if (!kTrain && rank == 0 && tid < rows) {
-            if (kSlots) decide_one<true>(B, ex_dev[slot], B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride, W.out_scale + n_frags);
+            if (kSlots) {
+                const int env = B.pending_list[list * B.n + row0 + tid];
+                decide_one<true>(B, ex_dev[slot], env, Y + tid * kYStride, W.out_scale + n_frags, env_eval && env_eval[env]);
+            }
             else decide_one(B, ex, B.pending_list[list * B.n + row0 + tid], Y + tid * kYStride);
         }
         stamp();         // 12: decisions applied
@@ -694,7 +703,7 @@ __global__ void __cluster_dims__(kFcCluster, 1, 1) __launch_bounds__(kFcThreads,
 trl_decide_fc_slots_kernel(Buffers B, PolicySlots P, const ExpSettings* __restrict__ ex_dev, const TRL_GRID_CONSTANT FcMaps maps,
                            const TRL_GRID_CONSTANT FcSlotMaps smaps, const int* __restrict__ tab, int* done_count, int list, int rearm) {
     const FwdTrain none{};
-    fc_stage<false, true>(B, *P.W, ex_dev, maps, none, done_count, list, rearm, &smaps, tab);
+    fc_stage<false, true>(B, *P.W, ex_dev, maps, none, done_count, list, rearm, &smaps, tab, P.env_eval);
 }
 // the FC stage over a trainer minibatch: activations and raw outputs to global memory, no decisions
 __global__ void __cluster_dims__(kFcCluster, 1, 1) __launch_bounds__(kFcThreads, 1)
@@ -738,9 +747,9 @@ void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSetti
 void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st) {
     TRL_LAUNCH(trl_cell_stats_kernel, (kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1), 1024, 0, st, B, env_slot, out);
 }
-void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot, double* out,
-                       cudaStream_t st) {
-    TRL_LAUNCH(trl_phys_stats_kernel, 1, 1024, 0, st, B, env_slot, env_phys, policy_slot, terrain_slot, phys_slot, out);
+void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot,
+                       const int* env_eval, int eval, double* out, cudaStream_t st) {
+    TRL_LAUNCH(trl_phys_stats_kernel, 1, 1024, 0, st, B, env_slot, env_phys, policy_slot, terrain_slot, phys_slot, env_eval, eval, out);
 }
 
 // the forward pass of a trainer minibatch through the same two kernels (trl_train.cu: enqueue_forward); act2 = [rows][5984] scratch the

@@ -80,6 +80,10 @@ struct trl_handle {
     std::vector<int> env_phys_host;                            // the assignment of every env (row 1 of env_phys)
     int* env_phys = nullptr;                                   // device [2][n]: slot of the present episode, slot from the next reset on
     double* phys_stats = nullptr;                              // [4] (trl_eval_stats_phys)
+    // evaluation envs (trl_set_env_eval, exploration handles only): until the first call env_eval is null, env_eval_host empty and
+    // every env explores.  From then on the decisions run the slot build (slots_active) and the step launches the physics-slot build
+    std::vector<int> env_eval_host;                            // the assignment of every env (row 1 of env_eval)
+    int* env_eval = nullptr;                                   // device [2][n]: mode of the present episode, mode from the next reset on
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
     bool use_graph = true;
@@ -122,6 +126,8 @@ extern "C" trl_handle* trl_create_common(trl_handle* h, int num_envs, int device
 int trl_drain(trl_handle* h);                         // every stream of the handle idle
 // terrain slot `slot` >= 1 holds parameter sets [n][40] of generator `type` (trl_load_terrain once the file is read)
 int trl_set_terrain_slot(trl_handle* h, int slot, int type, std::vector<double> sets);
+// the per-env modes of trl_set_env_eval, every env exploring, and the decision / step builds that read them (trl_host.cu)
+extern "C" int trl_enable_env_eval(trl_handle* h);
 
 // One array of a checkpoint (trl_checkpoint.cu): `bytes` of device memory at `dev`, or of host memory at `host` when dev is null.
 // `cap` is the room there is: a restore accepts up to cap bytes (the replay rows, the tuple block and the distance log are saved up

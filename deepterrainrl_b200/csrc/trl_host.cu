@@ -36,8 +36,8 @@ void launch_decide2(const Buffers& B, const NetWeights& W, const ExpSettings* ex
 void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSettings* ex, const FcMaps& maps, const FcSlotMaps& smaps, double* act2,
                           int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part);
 void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
-void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot, double* out,
-                       cudaStream_t st);
+void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot,
+                       const int* env_eval, int eval, double* out, cudaStream_t st);
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
@@ -49,10 +49,10 @@ void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStre
 // trl_step_ps_cg.cu); the emulator's trl / trl_cg builds are all of those
 #ifdef TRL_SIMT_EMU
 namespace trl {
-cudaError_t upload_phys(const PhysParams* phys, int* env_phys);
+cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval);
 }
 namespace trl_cg {
-cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 }
 namespace trl_ts = trl;
 namespace trl_ts_cg = trl_cg;
@@ -73,7 +73,7 @@ void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStre
 }  // namespace trl_ts_cg
 namespace trl_ps {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
-cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 void launch_reset(const trl::Buffers& B, const uint64_t* seeds, const int* env_ids, int count, int reseed, cudaStream_t st);
@@ -81,7 +81,7 @@ void launch_terrain(const trl::Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl_ps
 namespace trl_ps_cg {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
-cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_ps_cg
@@ -94,15 +94,15 @@ using namespace trl;
 struct trl_handle;
 static const trl_handle* g_model_owner = nullptr;    // whose ModelConst currently sits in the __constant__ copies
 static int g_device = -1;                             // the one device this process drives (set by the first handle)
-static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys) {
+static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys, int* env_eval) {
     cudaError_t e = trl::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ts::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ts_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ps::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ps_cg::upload_model(mc, terrain);
-    if (e == cudaSuccess) e = trl_ps::upload_phys(phys, env_phys);
-    return e != cudaSuccess ? e : trl_ps_cg::upload_phys(phys, env_phys);
+    if (e == cudaSuccess) e = trl_ps::upload_phys(phys, env_phys, env_eval);
+    return e != cudaSuccess ? e : trl_ps_cg::upload_phys(phys, env_phys, env_eval);
 }
 
 static thread_local std::string g_err;
@@ -137,7 +137,7 @@ static int ensure_model_only(trl_handle* h) {
     h->terrain[0].type = h->mc.terrain_type;      // slot 0 of the terrain table is the scene's own terrain
     std::memcpy(h->terrain[0].params, h->mc.terrain_params, sizeof(h->mc.terrain_params));
     h->phys[0] = h->mc.phys;                      // and slot 0 of the physics table its own physics
-    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys) != cudaSuccess) return 1;
+    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys, h->env_eval) != cudaSuccess) return 1;
     g_model_owner = h;
     return 0;
 }
@@ -528,10 +528,11 @@ static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, 
     else if (part & 1)
         launch_decide(h->B, h->W, h->d_ex, h->done_count, h->decide_grid, list, rearm, st);
 }
-// the env-step launches of a handle: the physics-slot builds once a physics slot is loaded (trl_load_physics; they serve terrain
-// slots too), else the terrain-slot builds once a terrain slot is loaded (trl_load_terrain), else the plain ones
+// the env-step launches of a handle: the physics-slot builds once a physics slot is loaded (trl_load_physics) or an env was given a
+// mode (trl_set_env_eval; they serve terrain slots too), else the terrain-slot builds once a terrain slot is loaded
+// (trl_load_terrain), else the plain ones
 static bool terrain_slots(const trl_handle* h) { return !h->env_terrain_host.empty(); }
-static bool phys_slots(const trl_handle* h) { return h->env_phys != nullptr; }
+static bool phys_slots(const trl_handle* h) { return h->env_phys != nullptr || h->env_eval != nullptr; }
 static void step_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1) {
     if (phys_slots(h)) trl_ps::launch_step(h->B, step, flags, lists, st, group, n_groups);
     else if (terrain_slots(h)) trl_ts::launch_step(h->B, step, flags, lists, st, group, n_groups);
@@ -1549,14 +1550,14 @@ int trl_env_physics(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
 }
 
 // a cell with any physics slot, or any cell of a handle whose envs are all on physics slot 0, is trl_eval_stats_cell's; the others come
-// from trl_phys_stats_kernel
-int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes, double* avg_dist,
-                        int64_t* env_steps) {
-    const std::string who = "trl_eval_stats_phys";
+// from trl_phys_stats_kernel.  env_eval (trl_eval_stats_mode): only the envs whose present episode has mode `eval` (1 evaluates)
+static int eval_stats_phys(trl_handle* h, const std::string& who, int policy_slot, int terrain_slot, int phys_slot, const int* env_eval, int eval,
+                           int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
     if (!h) return fail(who + ": null handle");
     if (phys_slot < -1 || phys_slot >= kMaxPhysSlots) return fail(who + ": physics slot " + std::to_string(phys_slot) + " out of range");
     if (phys_slot >= 0 && !phys_loaded(h, phys_slot)) return fail(who + ": physics slot " + std::to_string(phys_slot) + " is empty");
-    if (phys_slot < 0 || !h->env_phys) return eval_stats_cell(h, who.c_str(), policy_slot, terrain_slot, cycles, episodes, avg_dist, env_steps);
+    if (!env_eval && (phys_slot < 0 || !h->env_phys))
+        return eval_stats_cell(h, who.c_str(), policy_slot, terrain_slot, cycles, episodes, avg_dist, env_steps);
     if (policy_slot < -1 || policy_slot >= kMaxPolicySlots) return fail(who + ": policy slot " + std::to_string(policy_slot) + " out of range");
     if (policy_slot >= 0 && !slot_loaded(h, policy_slot)) return fail(who + ": policy slot " + std::to_string(policy_slot) + " is empty");
     if (terrain_slot < -1 || terrain_slot >= kMaxTerrainSlots) return fail(who + ": terrain slot " + std::to_string(terrain_slot) + " out of range");
@@ -1564,7 +1565,7 @@ int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int ph
     if (!h->phys_stats) CK(dalloc(h, &h->phys_stats, 4));
     double st[4];
     launch_phys_stats(h->B, h->slots_active ? h->P.env_slot : nullptr, h->env_phys, h->slots_active ? policy_slot : -1,
-                      h->env_terrain_host.empty() ? -1 : terrain_slot, phys_slot, h->phys_stats, h->stream);
+                      h->env_terrain_host.empty() ? -1 : terrain_slot, h->env_phys ? phys_slot : -1, env_eval, eval, h->phys_stats, h->stream);
     h->launches += 1;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(st, h->phys_stats, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
@@ -1574,6 +1575,89 @@ int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int ph
     if (env_steps) *env_steps = (int64_t)st[2];
     if (avg_dist) *avg_dist = st[1] > 0 ? st[3] / st[1] : 0.0;
     return 0;
+}
+
+int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes, double* avg_dist,
+                        int64_t* env_steps) {
+    return eval_stats_phys(h, "trl_eval_stats_phys", policy_slot, terrain_slot, phys_slot, nullptr, 0, cycles, episodes, avg_dist, env_steps);
+}
+
+// evaluation envs of an exploration handle: the per-env modes ([2][n]: present episode, next one), the slot build of the decision
+// kernels (which turns exploration off for an evaluating env) and the physics-slot build of the step kernels (which keeps an
+// evaluating env's episode statistics instead of its tuples).  Called with the handle drained; once made, they stay
+int trl_enable_env_eval(trl_handle* h) {
+    if (h->env_eval) return 0;
+    if (ensure_policy_slots(h)) return 1;
+    int* d = nullptr;
+    CK(dalloc(h, &d, 2 * (size_t)h->n));
+    h->env_eval = d;
+    h->env_eval_host.assign((size_t)h->n, 0);
+    h->P.env_eval = d;
+    h->slots_active = true;      // slot 0 alone: its table entry is bound to h->W (its trainer's net) by ensure_slot_tables
+    h->slot_dirty = true;
+    destroy_graphs(h);
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail("trl_set_env_eval: model upload failed") : 0;
+}
+
+int trl_set_env_eval(trl_handle* h, const int32_t* env_ids, const int32_t* flags, int n) {
+    const std::string who = "trl_set_env_eval";
+    if (!h) return fail(who + ": null handle");
+    if (h->mode != TRL_MODE_EXPLORE) return fail(who + ": every env of an evaluation handle evaluates (evaluation envs are for exploration handles)");
+    if (!h->mc.has_net) return fail(who + ": the scene has no policy net");
+    if (!h->decide_v2) return fail(who + ": the TRL_DECIDE_V1 decision kernel has no evaluation envs");
+    if (h->comm) return fail(who + ": evaluation envs do not run with a communicator");
+    if (n < 0 || n > h->n) return fail(who + ": env count out of range");
+    if (n > 0 && !flags) return fail(who + ": null flag list");
+    for (int k = 0; k < n; ++k) {
+        const int e = env_ids ? env_ids[k] : k;
+        if (e < 0 || e >= h->n) return fail(who + ": env id " + std::to_string(e) + " out of range");
+    }
+    if (drain(h) || trl_enable_env_eval(h)) return 1;
+    std::vector<int> next = h->env_eval_host;
+    for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = flags[k] ? 1 : 0;
+    CK(cudaMemcpy(h->env_eval + h->n, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
+    h->env_eval_host.swap(next);
+    return 0;
+}
+
+int trl_env_eval(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
+    if (!h) return fail("trl_env_eval: null handle");
+    if (n < 0 || n > h->n) return fail("trl_env_eval: env count out of range");
+    if (!h->env_eval) {
+        const int all = h->mode == TRL_MODE_POLI_EVAL ? 1 : 0;
+        for (int k = 0; k < n; ++k) {
+            if (current) current[k] = all;
+            if (assigned) assigned[k] = all;
+        }
+        return 0;
+    }
+    if (drain(h)) return 1;
+    if (current && n > 0) CK(cudaMemcpy(current, h->env_eval, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (assigned && n > 0) CK(cudaMemcpy(assigned, h->env_eval + h->n, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+// trl_eval_stats_phys over the envs whose present episode runs in `mode`; a handle whose envs all run in one mode gives that mode
+// every env and the other none
+int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
+                        double* avg_dist, int64_t* env_steps) {
+    const std::string who = "trl_eval_stats_mode";
+    if (!h) return fail(who + ": null handle");
+    if (mode != -1 && mode != TRL_MODE_POLI_EVAL && mode != TRL_MODE_EXPLORE)
+        return fail(who + ": mode " + std::to_string(mode) + " is none of TRL_MODE_POLI_EVAL, TRL_MODE_EXPLORE or -1 (any)");
+    if (mode == -1 || (!h->env_eval && mode == h->mode))
+        return eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, cycles, episodes, avg_dist, env_steps);
+    if (!h->env_eval) {     // no env runs in the other mode: the slots are checked, the figures are zero
+        if (eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, nullptr, nullptr, nullptr, nullptr)) return 1;
+        if (cycles) *cycles = 0;
+        if (episodes) *episodes = 0;
+        if (avg_dist) *avg_dist = 0.0;
+        if (env_steps) *env_steps = 0;
+        return 0;
+    }
+    return eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, h->env_eval, mode == TRL_MODE_POLI_EVAL ? 1 : 0, cycles, episodes,
+                           avg_dist, env_steps);
 }
 
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {

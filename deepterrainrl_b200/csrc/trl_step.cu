@@ -73,8 +73,13 @@ __constant__ TerrainSlot c_terrain[kMaxTerrainSlots];    // slot 0 = c_model's t
 __constant__ PhysParams c_phys[kMaxPhysSlots];   // slot 0 = c_model.phys (trl_types.h: kMaxPhysSlots)
 __constant__ int* c_env_phys;                    // [2][n] of the owning handle: the physics slot of every env's present episode, then
                                                  // the slot it gets at its next reset; null while the handle has no physics slot
+__constant__ int* c_env_eval;                    // [2][n] likewise the mode (1 evaluates, 0 explores) of the envs of an exploration
+                                                 // handle (trl_set_env_eval); null while no env has been given one
+// whether the present episode of `env` explores: every env of an exploration handle does, unless it has been set to evaluate
+__device__ __forceinline__ bool env_explores(int env) { return c_model.exp_mode && !(c_env_eval && c_env_eval[env]); }
 #else
 #define TRL_PHYS_TABLE 0
+__device__ __forceinline__ bool env_explores(int) { return c_model.exp_mode; }
 #endif
 // character-type branches: a run-time constant of the scene (the raptor's controller differs from the dog's / goat's); an experiment
 // build can fix it at compile time (-DTRL_FIXED_CHAR=0 dog / goat, 2 raptor) to see what the unused branches cost
@@ -1284,6 +1289,11 @@ __device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B
         }
 #if TRL_PHYS_TABLE
         if (c_env_phys) c_env_phys[L.env] = c_env_phys[(size_t)L.n + L.env];   // likewise the physics slot (trl_set_env_physics)
+        if (c_env_eval) {       // and the mode (trl_set_env_eval): evaluation counts cycles over episodes, from 0 when it begins
+            const int next = c_env_eval[(size_t)L.n + L.env];
+            if (next && !c_env_eval[L.env]) L.i(I_CYCLE_COUNT) = 0;
+            c_env_eval[L.env] = next;
+        }
 #endif
         GroundView g = load_ground(L, B);
         g.n[0] = g.n[1] = 0; g.flip = 0;
@@ -1292,7 +1302,7 @@ __device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B
         if (m.has_init_x) newx = m.init_x;
         newy = e.oy + g.sample(newx);
         store_ground(L, g);
-        if (m.exp_mode) {
+        if (env_explores(L.env)) {
             L.i(I_CYCLE_COUNT) = 0;
             L.i(I_CMD) = rng.rand_int(0, m.n_actions);   // cScenarioExp::CommandRandAction
         } else {
@@ -1461,7 +1471,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         if (lane == 0) { nc = (L.i(I_STATE) == 0 && L.d(D_PHASE) == 0.0) ? 1 : 0; fl = has_fallen(L, e.q) ? 1 : 0; }
         nc = shfi(nc, 0); fl = shfi(fl, 0);
         if (nc) {
-            if (m.exp_mode) exp_new_cycle_update(L, B, fl != 0, lane);
+            if (env_explores(env)) exp_new_cycle_update(L, B, fl != 0, lane);
             else if (lane == 0) L.i(I_CYCLE_COUNT) += 1;
         }
         TRL_CLK_END(PH_CTRL_REST, clk);
@@ -1473,7 +1483,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         if (lane == 0) { fallen = has_fallen(L, e.q) ? 1 : 0; new_cycle = (L.i(I_STATE) == 0 && L.d(D_PHASE) == 0.0) ? 1 : 0; }
         fallen = shfi(fallen, 0); new_cycle = shfi(new_cycle, 0);
         bool do_reset = false;
-        if (m.exp_mode) {
+        if (env_explores(env)) {     // the ending episode's own mode: reset_env then gives the next one its assigned mode
             if (!new_cycle && fallen) { exp_new_cycle_update(L, B, true, lane); do_reset = true; }
         } else if (fallen) {
             if (lane == 0 && L.i(I_CYCLE_COUNT) >= 1) {
@@ -1698,10 +1708,12 @@ cudaError_t upload_model(const ModelConst& mc, const TerrainSlot* terrain) {
     return e;
 }
 #if TRL_PHYS_TABLE
-// the physics table (slot 0 = mc.phys) and the handle's per-env slot array (null: every env on slot 0), uploaded with the model
-cudaError_t upload_phys(const PhysParams* phys, int* env_phys) {
+// the physics table (slot 0 = mc.phys), the handle's per-env slot array (null: every env on slot 0) and per-env mode array (null: every
+// env in the handle's mode), uploaded with the model
+cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval) {
     cudaError_t e = cudaMemcpyToSymbol(c_phys, phys, sizeof(PhysParams) * kMaxPhysSlots);
     if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_phys, &env_phys, sizeof(env_phys));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_eval, &env_eval, sizeof(env_eval));
     return e;
 }
 #endif

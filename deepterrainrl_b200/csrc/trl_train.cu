@@ -1079,7 +1079,7 @@ trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* p, c
     if (slot < 0 || slot >= kMaxPolicySlots) return refuse("trl_trainer_create_slot: slot " + std::to_string(slot) + " out of range (0.." + std::to_string(kMaxPolicySlots - 1) + ")");
     if (slot == 0) {
         if (h->trainer) return refuse("trl_trainer_create: a trainer is already attached");
-        if (h->slots_active && !h->train_slots)
+        if (h->slots_active && !h->train_slots && h->mode == TRL_MODE_POLI_EVAL)
             return refuse("trl_trainer_create: the handle evaluates several policy slots (trl_load_policy); a trainer needs a single-policy handle");
     } else {
         if (h->mode != TRL_MODE_EXPLORE) return refuse("trl_trainer_create_slot: training slots are for exploration handles (TRL_MODE_EXPLORE)");

@@ -203,6 +203,7 @@ struct PolicySlots {
     int* sort_tmp;           // [lag][n]  copy of a pending list while it is regrouped by slot
     int* chunks;             // [lag][1 + 3 * chunk_cap]  {number of chunks, then {slot, row0, rows} per 32-row FC chunk}
     int chunk_cap;           // n / 32 + kMaxPolicySlots: every slot's ragged last chunk included
+    const int* env_eval;     // [2][n]  mode of each env's present episode (row 0; 1 evaluates) and next one (trl_set_env_eval), or null
 };
 
 // Device buffers of one batch of environments.

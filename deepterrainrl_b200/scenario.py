@@ -137,6 +137,7 @@ EXPORTS = [
     "trl_set_explore_slot", "trl_train_run_slots_sched",
     "trl_checkpoint_save", "trl_create_from_checkpoint", "trl_trainer_params", "trl_env_policy",
     "trl_load_physics", "trl_set_env_physics", "trl_env_physics", "trl_eval_stats_phys",
+    "trl_set_env_eval", "trl_env_eval", "trl_eval_stats_mode",
 ]
 
 
@@ -311,6 +312,22 @@ class BatchedScenario:
         self._ck(self.L.trl_env_physics(self.h, _p(cur), _p(nxt), self.num_envs))
         return cur, nxt
 
+    def SetEnvEval(self, flags, env_ids=None):
+        """env_ids[k] (default: env k) of an exploration scenario evaluates its policy slot's current net, exploration off and no
+        tuples recorded, from its next episode reset on if flags[k] is true; it explores again from its next reset if false"""
+        f = np.ascontiguousarray(flags, dtype=np.int32).ravel()
+        ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        if ids is not None and ids.size != f.size:
+            raise ValueError("SetEnvEval: one flag per env id")
+        self._ck(self.L.trl_set_env_eval(self.h, _p(ids), _p(f), int(f.size)))
+
+    def EnvEval(self):
+        """(current, assigned): per env, whether its present episode evaluates and whether the one after its next reset will"""
+        cur = np.zeros(self.num_envs, np.int32)
+        nxt = np.zeros(self.num_envs, np.int32)
+        self._ck(self.L.trl_env_eval(self.h, _p(cur), _p(nxt), self.num_envs))
+        return cur.astype(bool), nxt.astype(bool)
+
     def GetOutputOffsetScale(self):
         """cBaseControllerMACE::BuildNNOutputOffsetScale."""
         n = self.num_frags * (1 + self.frag_size)
@@ -461,11 +478,15 @@ class BatchedScenario:
     def GetNumEnvSteps(self):
         return self._stats()["steps"]
 
-    def GetEvalStats(self, slot=0, terrain=None, physics=None):
+    def GetEvalStats(self, slot=0, terrain=None, physics=None, mode=None):
         """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot` (None: any) whose present ground comes from
-        terrain slot `terrain` (None: any) and whose present episode runs on physics slot `physics` (None: any)"""
+        terrain slot `terrain` (None: any), whose present episode runs on physics slot `physics` (None: any) and in mode `mode`
+        (TRL_MODE_POLI_EVAL = 0 evaluates, TRL_MODE_EXPLORE = 1 explores; None: any)"""
         c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
-        if physics is not None:
+        if mode is not None:
+            rc = self.L.trl_eval_stats_mode(self.h, int(mode), -1 if slot is None else int(slot), -1 if terrain is None else int(terrain),
+                                            -1 if physics is None else int(physics), C.byref(c), C.byref(e), C.byref(a), C.byref(s))
+        elif physics is not None:
             rc = self.L.trl_eval_stats_phys(self.h, -1 if slot is None else int(slot), -1 if terrain is None else int(terrain), int(physics),
                                             C.byref(c), C.byref(e), C.byref(a), C.byref(s))
         elif terrain is None and slot is not None:
@@ -476,9 +497,12 @@ class BatchedScenario:
         self._ck(rc)
         return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
 
-    def GetDistLog(self, slot=None, terrain=None, physics=None):
-        """(distances, env ids) of the episodes logged so far; slot / terrain / physics: only the entries of envs now on that policy slot
-        / whose present ground comes from that terrain slot / whose present episode runs on that physics slot"""
+    def GetDistLog(self, slot=None, terrain=None, physics=None, mode=None):
+        """(distances, env ids) of the episodes logged so far; slot / terrain / physics / mode: only the entries of envs now on that
+        policy slot / whose present ground comes from that terrain slot / whose present episode runs on that physics slot / whose
+        present episode runs in that mode (0 evaluates, 1 explores).  Every filter reads the env's present assignment, not the one of
+        the logged episode: only evaluating episodes log a distance, but an env that has gone back to exploring keeps its entries,
+        which mode=1 then returns and mode=0 drops."""
         d = C.c_void_p(); e = C.c_void_p(); n = C.c_int(0)
         self._ck(self.L.trl_dist_log(self.h, C.byref(d), C.byref(e), C.byref(n)))
         if n.value == 0:
@@ -493,6 +517,9 @@ class BatchedScenario:
             dist, env = dist[keep], env[keep]
         if physics is not None:
             keep = self.EnvPhysics()[0][env] == physics
+            dist, env = dist[keep], env[keep]
+        if mode is not None:
+            keep = self.EnvEval()[0][env] == (int(mode) == 0)
             dist, env = dist[keep], env[keep]
         return dist, env
 

@@ -165,7 +165,18 @@ def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step
     iters_per_update: the iterations of every trainer per update (lock-step; the schedules are read at the iterations done in this
     call); None = each trainer paced as in ScenarioTrainMACE: one iteration per `tuple_buffer_size` fresh tuples of its slot, its
     schedule read at its own iteration count.  One schedule with a fixed count is trl_train_run_slots (applied handle-wide); every
-    other call is trl_train_run_slots_sched."""
+    other call is trl_train_run_slots_sched.
+
+    A learning curve per slot, from evaluation envs of the same scenario (they run their slot's current net, exploration off, and
+    feed no trainer)::
+
+        ex.SetEnvEval(np.arange(ex.num_envs) % 8 == 0)     # every 8th env evaluates from its next episode on
+        ex.Reset()
+        curve = []
+        for _ in range(blocks):
+            train_run_slots(trainers, schedules, 10, None)
+            curve.append([ex.GetEvalStats(slot=t.slot, mode=0)["avg_dist"] for t in trainers])
+            ex.ResetAvgDist()"""
     trainers = list(trainers)
     if not trainers:
         raise ValueError("train_run_slots: no trainer")

@@ -225,6 +225,28 @@ int trl_set_env_physics(trl_handle* h, const int32_t* env_ids, const int32_t* sl
 int trl_env_physics(trl_handle* h, int32_t* current, int32_t* assigned, int n);
 int trl_eval_stats_phys(trl_handle* h, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
                         double* avg_dist, int64_t* env_steps);
+/* Evaluation envs (exploration handles, with or without trainers, training, terrain or physics slots): an env set to evaluate runs its
+ * policy slot's current net (its trainer's, if the slot has one) with exploration off, records no tuples, and keeps the episode and
+ * distance statistics of an evaluation handle.  Its slot's trainer goes on training from the slot's exploring envs.  With the same
+ * seeds, an evaluating env j on policy slot p computes bit for bit what env j computes in a TRL_MODE_POLI_EVAL handle on the same
+ * terrain / physics slot whose net is, before every update, the one slot p holds then -- except the counter-RNG position
+ * (I_RNG_CTR_LO/HI): evaluation decisions draw a number they do not use, and earlier exploring episodes moved the counter.  An exploring
+ * env computes what it computes in the same handle without evaluation envs; each trainer is fed only its slot's exploring envs' tuples.
+ *   trl_set_env_eval    env_ids[k] (NULL: env k) evaluates from its next episode if flags[k] != 0, explores otherwise; every env starts
+ *                       exploring.  Takes effect at the env's next episode reset (a fall inside trl_update, trl_reset,
+ *                       trl_seed_terrain): the ending episode's bookkeeping follows its own mode, and an episode never mixes two.  Entering
+ *                       evaluation restarts the env's cycle count at 0; episodes and mean distance accumulate over its evaluating
+ *                       episodes until trl_reset_avg_dist.  Refused, handle unchanged, for an evaluation handle, a scene without a policy
+ *                       net, the TRL_DECIDE_V1 build, a handle with a communicator (trl_comm_init* refuses a handle with evaluation
+ *                       envs), an env id out of range or n > num_envs.
+ *   trl_env_eval        per env (first n), 1 if its present episode evaluates, and the same for the mode it gets at its next reset.
+ *   trl_eval_stats_mode trl_eval_stats_phys(policy_slot, terrain_slot, phys_slot) over the envs whose present episode runs in `mode`
+ *                       (TRL_MODE_POLI_EVAL, TRL_MODE_EXPLORE, -1 = any); (-1, p, t, q) is trl_eval_stats_phys(p, t, q).  The other
+ *                       statistics entries keep counting every env. */
+int trl_set_env_eval(trl_handle* h, const int32_t* env_ids, const int32_t* flags, int n);
+int trl_env_eval(trl_handle* h, int32_t* current, int32_t* assigned, int n);
+int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
+                        double* avg_dist, int64_t* env_steps);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
