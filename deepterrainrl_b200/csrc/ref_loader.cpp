@@ -77,28 +77,26 @@ TerrainFile read_terrain_file(const std::string& path) {
     return tf;
 }
 
-void build_scene_from_args(int argc, const char* const* argv, const std::string& root, ScenePack* out) {
-    // CLI tokens first, then the arg file's, so the CLI wins on first-match lookup (optimizer/Main.cpp:19-32)
-    ArgList args;
-    args.append_args(argc, argv);
-    std::string arg_file;
-    if (args.find("arg_file", &arg_file)) args.append_file(join(root, arg_file));
+std::string join_path(const std::string& root, const std::string& rel) { return join(root, rel); }
 
-    const std::string char_file = args.str("character_file", "");
-    if (char_file.empty()) throw std::runtime_error("No character file specified.");
-    const int char_type = index_of(kCharNames, args.str("char_type", "none"), "char_type");
-    const int ctrl = index_of(kCtrlNames, args.str("char_ctrl", "none"), "char_ctrl");
-    const bool raptor = char_type == 2;
-    JValue ch = load_json(join(root, char_file));
-
+CharacterRecords read_character_file(const std::string& path, const std::string& root, bool raptor, int expect_nj) {
+    JValue ch = load_json(path);
     const JValue* skel = ch.get("Skeleton");
     const JValue* joints = skel ? skel->get("Joints") : nullptr;
     const JValue* bodies = ch.get("BodyDefs");
     const JValue* pds = ch.get("PDControllers");
     const JValue* ctrls = ch.get("Controllers");
     if (!joints || !bodies || !pds || !ctrls) throw std::runtime_error("character file misses Skeleton / BodyDefs / PDControllers / Controllers");
+    CharacterRecords cr;
     const int nj = (int)joints->arr.size();
-    std::vector<double> J(7 * nj), B(9 * nj), P(6 * nj);
+    if (expect_nj >= 0 && nj != expect_nj)
+        throw std::runtime_error("the character's topology differs from the scene's: " + std::to_string(nj) + " joints, the scene's character has " +
+                                 std::to_string(expect_nj));
+    if (bodies->arr.size() < (size_t)nj || pds->arr.size() < (size_t)nj)
+        throw std::runtime_error("character file has fewer BodyDefs / PDControllers than joints");
+    cr.nj = nj;
+    std::vector<double>&J = cr.joints, &B = cr.bodies, &P = cr.pd;
+    J.assign(7 * nj, 0.0); B.assign(9 * nj, 0.0); P.assign(6 * nj, 0.0);
     int ndof = 0;
     for (int i = 0; i < nj; ++i) {
         const JValue& j = joints->arr[i];
@@ -119,20 +117,42 @@ void build_scene_from_args(int argc, const char* const* argv, const std::string&
         w[0] = p.number("Kp", 0); w[1] = p.number("Kd", 0); w[2] = p.number("TorqueLim", 0); w[3] = p.number("TargetTheta", 0);
         w[4] = p.number("TargetVel", 0); w[5] = p.number("UseWorldCoord", 0);
     }
-    J[2] = J[3] = J[4] = 0.0;   // PostProcessJointMat zeroes the root attach point (anim/KinTree.cpp:1004-1016)
+    if (nj > 0) J[2] = J[3] = J[4] = 0.0;   // PostProcessJointMat zeroes the root attach point (anim/KinTree.cpp:1004-1016)
+    cr.ndof = ndof;
 
-    std::vector<double> C, A;
     const JValue* files = ctrls->get("Files");
     const JValue* actions = ctrls->get("Actions");
-    int n_ctrl = 0, n_actions = 0;
-    if (files) for (const JValue& f : files->arr) { std::vector<double> v = read_ctrl_params(join(root, f.str), raptor); C.insert(C.end(), v.begin(), v.end()); ++n_ctrl; }
-    if (actions) for (const JValue& a : actions->arr) {
-        A.push_back(a.number("ParamIdx0", 0)); A.push_back(a.number("ParamIdx1", 0)); A.push_back(a.number("Blend", 0)); A.push_back(a.number("Cyclic", 0));
-        ++n_actions;
+    if (files) for (const JValue& f : files->arr) {
+        std::vector<double> v = read_ctrl_params(join(root, f.str), raptor);
+        cr.ctrl_params.insert(cr.ctrl_params.end(), v.begin(), v.end());
+        ++cr.n_ctrl;
     }
-    const int default_action = (int)ctrls->number("DefaultAction", 0);
-    const int grav_comp = ctrls->number("EnableGravityCompensation", 1) != 0 ? 1 : 0;
-    const int virt_forces = ctrls->number("EnableVirtualForces", 1) != 0 ? 1 : 0;
+    if (actions) for (const JValue& a : actions->arr) {
+        for (const char* k : {"ParamIdx0", "ParamIdx1", "Blend", "Cyclic"}) cr.actions.push_back(a.number(k, 0));
+        ++cr.n_actions;
+    }
+    cr.default_action = (int)ctrls->number("DefaultAction", 0);
+    cr.grav_comp = ctrls->number("EnableGravityCompensation", 1) != 0 ? 1 : 0;
+    cr.virt_forces = ctrls->number("EnableVirtualForces", 1) != 0 ? 1 : 0;
+    return cr;
+}
+
+void build_scene_from_args(int argc, const char* const* argv, const std::string& root, ScenePack* out) {
+    // CLI tokens first, then the arg file's, so the CLI wins on first-match lookup (optimizer/Main.cpp:19-32)
+    ArgList args;
+    args.append_args(argc, argv);
+    std::string arg_file;
+    if (args.find("arg_file", &arg_file)) args.append_file(join(root, arg_file));
+
+    const std::string char_file = args.str("character_file", "");
+    if (char_file.empty()) throw std::runtime_error("No character file specified.");
+    const int char_type = index_of(kCharNames, args.str("char_type", "none"), "char_type");
+    const int ctrl = index_of(kCtrlNames, args.str("char_ctrl", "none"), "char_ctrl");
+    const bool raptor = char_type == 2;
+    const CharacterRecords cr = read_character_file(join(root, char_file), root, raptor);
+    const int nj = cr.nj, ndof = cr.ndof, n_ctrl = cr.n_ctrl, n_actions = cr.n_actions;
+    const int default_action = cr.default_action, grav_comp = cr.grav_comp, virt_forces = cr.virt_forces;
+    const std::vector<double>&J = cr.joints, &B = cr.bodies, &P = cr.pd, &C = cr.ctrl_params, &A = cr.actions;
 
     std::vector<double> pose0(ndof, 0.0), vel0(ndof, 0.0);
     const std::string state_file = args.str("state_file", "");

@@ -305,6 +305,18 @@ private:
 // arg file refer to (the DeepTerrainRL checkout).  Mirrors tools/pack_scene.py record for record.
 void build_scene_from_args(int argc, const char* const* argv, const std::string& root, ScenePack* out);
 
+// The records of a character file (`-character_file`) as the scene pack stores them: joints [nj][7], bodies [nj][9], pd [nj][6], the
+// parameter sets of the controller files its Controllers section names (resolved against `root`, read for the raptor's layout when
+// `raptor`) [n_ctrl][n_params], actions [n_actions][4], and the Controllers flags.  Throws on a malformed file, and (expect_nj >= 0)
+// on a joint count other than expect_nj before any controller file is read.
+struct CharacterRecords {
+    int nj = 0, ndof = 0, n_ctrl = 0, n_actions = 0, default_action = 0, grav_comp = 1, virt_forces = 1;
+    std::vector<double> joints, bodies, pd, ctrl_params, actions;
+};
+CharacterRecords read_character_file(const std::string& path, const std::string& root, bool raptor, int expect_nj = -1);
+// path relative to root (absolute paths as given)
+std::string join_path(const std::string& root, const std::string& rel);
+
 // A terrain file (`-terrain_file`, cTerrainGen2D::LoadParams: {"Type": ..., "Params": [{...}, ...]}): the generator type and
 // n_sets parameter sets of 40 each, every parameter a file does not name at its cTerrainGen2D default.  Throws on an unknown type
 // or a malformed file.

@@ -194,6 +194,10 @@ int handle_state(trl_handle* h, std::vector<CkptSection>* out) {
         host("env_eval_host", 1, h->env_eval_host.data(), n * 4);
         fixed("env_eval", 1, h->env_eval, 2 * n * 4);
     }
+    if (h->env_body) {       // body slots: likewise written only once one is loaded
+        host("env_body_host", 1, h->env_body_host.data(), n * 4);
+        fixed("env_body", 1, h->env_body, 2 * n * 4);
+    }
     fixed("B.d", 3, B.d, (size_t)D_NUM_FIELDS * n * 8);
     fixed("B.i", 1, B.i, (size_t)I_NUM_PLANES * n * 4);
     fixed("B.terrain", 2, B.terrain, n * 2 * kTerrainCap * 4);
@@ -297,6 +301,13 @@ int save_impl(trl_handle* h, const char* path, const void* user, size_t user_byt
     if (h->env_eval) {
         const int32_t on = 1;
         build.push_back(blob_of("eval_envs", 1, &on, 1));
+    }
+    if (h->env_body) {
+        int32_t mask = 0;
+        for (int s = 1; s < kMaxBodySlots; ++s)
+            if (h->body_loaded[s]) mask |= 1 << s;
+        build.push_back(blob_of("body_loaded", 1, &mask, 1));
+        build.push_back(blob_of("body_table", 0, h->body, kMaxBodySlots));
     }
     build.insert(build.begin() + 1, blob_of("meta", 0, &m, 1));
     build.push_back(blob_of("user", 0, (const unsigned char*)user, user_bytes));
@@ -442,6 +453,16 @@ trl_handle* load_impl(const char* path, int device, trl_trainer** trainers_out, 
             const double p7[7] = {q.kn, q.dn, q.mu, q.v_eps, q.contact_tol, q.k_lim, q.d_lim};
             if (trl_load_physics(h, s, p7, q.vertex_contacts)) return bail("");
         }
+    }
+    if (const auto* lb = need("body_loaded", 0)) {     // the body slots from the stored tables (the files may be gone)
+        const auto* tb = need("body_table", sizeof(BodyConst) * kMaxBodySlots);
+        int32_t mask = 0;
+        if (lb->size() == 4) std::memcpy(&mask, lb->data(), 4);
+        if (!tb || lb->size() != 4 || mask == 0 || (mask & ~0xfe)) return bail("body slots: table or slot mask missing or malformed");
+        std::vector<BodyConst> table(kMaxBodySlots);
+        std::memcpy(table.data(), tb->data(), sizeof(BodyConst) * kMaxBodySlots);
+        for (int s = 1; s < kMaxBodySlots; ++s)
+            if ((mask & (1 << s)) && trl_set_body_slot(h, s, table[s])) return bail("");
     }
     if ((m.policies || m.trainers || eb) && !h->mc.has_net) return bail("the scene has no policy net");
     if (eb && trl_enable_env_eval(h)) return bail("");

@@ -292,9 +292,11 @@ __global__ void __launch_bounds__(1024) trl_cell_stats_kernel(Buffers B, const i
 
 // the same four figures over the envs of one (policy slot, terrain slot, physics slot) cell into out[4], -1 = any slot; one CTA with
 // trl_stats_kernel's traversal and reduction order.  The physics slot is the one of the env's present episode (env_phys row 0).
-// env_eval (optional, null: any mode): only the envs whose present episode's mode (row 0 of trl_set_env_eval's array) is `eval`
+// env_eval (optional, null: any mode): only the envs whose present episode's mode (row 0 of trl_set_env_eval's array) is `eval`;
+// env_body (optional, null: any body) likewise only the envs whose present episode runs on body slot `b` (row 0 of env_body)
 __global__ void __launch_bounds__(1024) trl_phys_stats_kernel(Buffers B, const int* __restrict__ env_slot, const int* __restrict__ env_phys, int p,
-                                                              int t, int q, const int* __restrict__ env_eval, int eval, double* __restrict__ out) {
+                                                              int t, int q, const int* __restrict__ env_eval, int eval,
+                                                              const int* __restrict__ env_body, int b, double* __restrict__ out) {
     __shared__ double red[4][32];
     const int w = threadIdx.x >> 5, l = threadIdx.x & 31, nw = blockDim.x >> 5;
     const int* terrain_slot = B.i + (size_t)I_TERRAIN_SLOT * B.n;
@@ -304,6 +306,7 @@ __global__ void __launch_bounds__(1024) trl_phys_stats_kernel(Buffers B, const i
         if (t >= 0 && terrain_slot[env] != t) continue;
         if (q >= 0 && env_phys[env] != q) continue;
         if (env_eval && env_eval[env] != eval) continue;
+        if (env_body && env_body[env] != b) continue;
         const int ec = B.i[(size_t)I_EPISODE_COUNT * B.n + env];
         c += B.i[(size_t)I_CYCLE_COUNT * B.n + env];
         e += ec;
@@ -748,8 +751,9 @@ void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaS
     TRL_LAUNCH(trl_cell_stats_kernel, (kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1), 1024, 0, st, B, env_slot, out);
 }
 void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot,
-                       const int* env_eval, int eval, double* out, cudaStream_t st) {
-    TRL_LAUNCH(trl_phys_stats_kernel, 1, 1024, 0, st, B, env_slot, env_phys, policy_slot, terrain_slot, phys_slot, env_eval, eval, out);
+                       const int* env_eval, int eval, const int* env_body, int body_slot, double* out, cudaStream_t st) {
+    TRL_LAUNCH(trl_phys_stats_kernel, 1, 1024, 0, st, B, env_slot, env_phys, policy_slot, terrain_slot, phys_slot, env_eval, eval, env_body,
+               body_slot, out);
 }
 
 // the forward pass of a trainer minibatch through the same two kernels (trl_train.cu: enqueue_forward); act2 = [rows][5984] scratch the

@@ -84,6 +84,14 @@ struct trl_handle {
     // every env explores.  From then on the decisions run the slot build (slots_active) and the step launches the physics-slot build
     std::vector<int> env_eval_host;                            // the assignment of every env (row 1 of env_eval)
     int* env_eval = nullptr;                                   // device [2][n]: mode of the present episode, mode from the next reset on
+    // body slots (trl_load_body, any mode): slot 0 is the scene's body (the per-link numbers of mc), copied into body[0] at every upload;
+    // slots 1.. hold bodies loaded from character files of the scene's topology.  body[] is the table of the body-slot build.  Until a
+    // slot >= 1 is loaded env_body is null, env_body_host empty, every env on slot 0, and the step launches run the other builds
+    trl::BodyConst body[trl::kMaxBodySlots] = {};
+    bool body_loaded[trl::kMaxBodySlots] = {};                 // [0] unused
+    std::vector<int> env_body_host;                            // the assignment of every env (row 1 of env_body)
+    int* env_body = nullptr;                                   // device [2][n]: slot of the present episode, slot from the next reset on
+    std::string data_root;                                     // trl_create's: the directory relative character and controller paths refer to
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
     bool use_graph = true;
@@ -128,6 +136,8 @@ int trl_drain(trl_handle* h);                         // every stream of the han
 int trl_set_terrain_slot(trl_handle* h, int slot, int type, std::vector<double> sets);
 // the per-env modes of trl_set_env_eval, every env exploring, and the decision / step builds that read them (trl_host.cu)
 extern "C" int trl_enable_env_eval(trl_handle* h);
+// body slot `slot` >= 1 holds `b` (trl_load_body once the file is read and checked), and the handle moves onto the body-slot build
+extern "C" int trl_set_body_slot(trl_handle* h, int slot, const trl::BodyConst& b);
 
 // One array of a checkpoint (trl_checkpoint.cu): `bytes` of device memory at `dev`, or of host memory at `host` when dev is null.
 // `cap` is the room there is: a restore accepts up to cap bytes (the replay rows, the tuple block and the distance log are saved up

@@ -37,7 +37,7 @@ void launch_decide2_slots(const Buffers& B, const PolicySlots& P, const ExpSetti
                           int* tmp, int* tab, int* done_count, int grid, int fc_clusters, int list, int rearm, cudaStream_t st, int part);
 void launch_cell_stats(const Buffers& B, const int* env_slot, double* out, cudaStream_t st);
 void launch_phys_stats(const Buffers& B, const int* env_slot, const int* env_phys, int policy_slot, int terrain_slot, int phys_slot,
-                       const int* env_eval, int eval, double* out, cudaStream_t st);
+                       const int* env_eval, int eval, const int* env_body, int body_slot, double* out, cudaStream_t st);
 void launch_terrain(const Buffers& B, double lookahead, cudaStream_t st);
 }  // namespace trl
 namespace trl_cg {
@@ -45,19 +45,23 @@ cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terr
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_cg
-// the terrain-slot builds of the env-step kernels (trl_step_ts.cu, trl_step_ts_cg.cu) and the physics-slot builds (trl_step_ps.cu,
-// trl_step_ps_cg.cu); the emulator's trl / trl_cg builds are all of those
+// the terrain-slot builds of the env-step kernels (trl_step_ts.cu, trl_step_ts_cg.cu), the physics-slot builds (trl_step_ps.cu,
+// trl_step_ps_cg.cu) and the body-slot builds (trl_step_bs.cu, trl_step_bs_cg.cu); the emulator's trl / trl_cg builds are all of those
 #ifdef TRL_SIMT_EMU
 namespace trl {
 cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval);
+cudaError_t upload_body(const BodyConst* body, int* env_body);
 }
 namespace trl_cg {
 cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
+cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
 }
 namespace trl_ts = trl;
 namespace trl_ts_cg = trl_cg;
 namespace trl_ps = trl;
 namespace trl_ps_cg = trl_cg;
+namespace trl_bs = trl;
+namespace trl_bs_cg = trl_cg;
 #else
 namespace trl_ts {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
@@ -85,6 +89,22 @@ cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eva
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_ps_cg
+namespace trl_bs {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
+cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+void launch_reset(const trl::Buffers& B, const uint64_t* seeds, const int* env_ids, int count, int reseed, cudaStream_t st);
+void launch_terrain(const trl::Buffers& B, double lookahead, cudaStream_t st);
+}  // namespace trl_bs
+namespace trl_bs_cg {
+cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
+cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
+cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
+cudaError_t configure_step_kernels();
+void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
+}  // namespace trl_bs_cg
 #endif
 
 
@@ -94,7 +114,8 @@ using namespace trl;
 struct trl_handle;
 static const trl_handle* g_model_owner = nullptr;    // whose ModelConst currently sits in the __constant__ copies
 static int g_device = -1;                             // the one device this process drives (set by the first handle)
-static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys, int* env_eval) {
+static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys, int* env_eval,
+                                    const BodyConst* body, int* env_body) {
     cudaError_t e = trl::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ts::upload_model(mc, terrain);
@@ -102,7 +123,29 @@ static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* ter
     if (e == cudaSuccess) e = trl_ps::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ps_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ps::upload_phys(phys, env_phys, env_eval);
-    return e != cudaSuccess ? e : trl_ps_cg::upload_phys(phys, env_phys, env_eval);
+    if (e == cudaSuccess) e = trl_ps_cg::upload_phys(phys, env_phys, env_eval);
+#ifndef TRL_SIMT_EMU
+    if (e == cudaSuccess) e = trl_bs::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_bs_cg::upload_model(mc, terrain);
+    if (e == cudaSuccess) e = trl_bs::upload_phys(phys, env_phys, env_eval);
+    if (e == cudaSuccess) e = trl_bs_cg::upload_phys(phys, env_phys, env_eval);
+#endif
+    if (e == cudaSuccess) e = trl_bs::upload_body(body, env_body);
+    return e != cudaSuccess ? e : trl_bs_cg::upload_body(body, env_body);
+}
+
+// the per-link numbers of the scene's body (slot 0 of the body table), as fill_model derived them from the character file
+static BodyConst body_of(const ModelConst& m) {
+    BodyConst b;
+    std::memset(&b, 0, sizeof(b));
+#define TRL_BODY_COPY(f) std::memcpy(&b.f, &m.f, sizeof(b.f))
+    TRL_BODY_COPY(attach_x); TRL_BODY_COPY(attach_y); TRL_BODY_COPY(lim_lo); TRL_BODY_COPY(lim_hi); TRL_BODY_COPY(has_limit);
+    TRL_BODY_COPY(mass); TRL_BODY_COPY(body_ax); TRL_BODY_COPY(body_ay); TRL_BODY_COPY(body_theta); TRL_BODY_COPY(body_cos);
+    TRL_BODY_COPY(body_sin); TRL_BODY_COPY(half_x); TRL_BODY_COPY(half_y); TRL_BODY_COPY(izz_o); TRL_BODY_COPY(izz_c);
+    TRL_BODY_COPY(corner_lx); TRL_BODY_COPY(corner_ly); TRL_BODY_COPY(kp); TRL_BODY_COPY(kd); TRL_BODY_COPY(torque_lim);
+    TRL_BODY_COPY(target_theta0); TRL_BODY_COPY(target_vel); TRL_BODY_COPY(world_pd); TRL_BODY_COPY(total_mass); TRL_BODY_COPY(reach);
+#undef TRL_BODY_COPY
+    return b;
 }
 
 static thread_local std::string g_err;
@@ -137,7 +180,8 @@ static int ensure_model_only(trl_handle* h) {
     h->terrain[0].type = h->mc.terrain_type;      // slot 0 of the terrain table is the scene's own terrain
     std::memcpy(h->terrain[0].params, h->mc.terrain_params, sizeof(h->mc.terrain_params));
     h->phys[0] = h->mc.phys;                      // and slot 0 of the physics table its own physics
-    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys, h->env_eval) != cudaSuccess) return 1;
+    h->body[0] = body_of(h->mc);                  // and slot 0 of the body table its own body
+    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys, h->env_eval, h->body, h->env_body) != cudaSuccess) return 1;
     g_model_owner = h;
     return 0;
 }
@@ -528,28 +572,34 @@ static void enqueue_decide(trl_handle* h, int list, int rearm, cudaStream_t st, 
     else if (part & 1)
         launch_decide(h->B, h->W, h->d_ex, h->done_count, h->decide_grid, list, rearm, st);
 }
-// the env-step launches of a handle: the physics-slot builds once a physics slot is loaded (trl_load_physics) or an env was given a
+// the env-step launches of a handle: the body-slot builds once a body slot is loaded (trl_load_body; they serve terrain and physics
+// slots and evaluation envs too), else the physics-slot builds once a physics slot is loaded (trl_load_physics) or an env was given a
 // mode (trl_set_env_eval; they serve terrain slots too), else the terrain-slot builds once a terrain slot is loaded
 // (trl_load_terrain), else the plain ones
 static bool terrain_slots(const trl_handle* h) { return !h->env_terrain_host.empty(); }
 static bool phys_slots(const trl_handle* h) { return h->env_phys != nullptr || h->env_eval != nullptr; }
+static bool body_slots(const trl_handle* h) { return h->env_body != nullptr; }
 static void step_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1) {
-    if (phys_slots(h)) trl_ps::launch_step(h->B, step, flags, lists, st, group, n_groups);
+    if (body_slots(h)) trl_bs::launch_step(h->B, step, flags, lists, st, group, n_groups);
+    else if (phys_slots(h)) trl_ps::launch_step(h->B, step, flags, lists, st, group, n_groups);
     else if (terrain_slots(h)) trl_ts::launch_step(h->B, step, flags, lists, st, group, n_groups);
     else launch_step(h->B, step, flags, lists, st, group, n_groups);
 }
 static void catchup_launch(const trl_handle* h, double step, int flags, int lists, cudaStream_t st) {
-    if (phys_slots(h)) trl_ps_cg::launch_step(h->B, step, flags, lists, st);
+    if (body_slots(h)) trl_bs_cg::launch_step(h->B, step, flags, lists, st);
+    else if (phys_slots(h)) trl_ps_cg::launch_step(h->B, step, flags, lists, st);
     else if (terrain_slots(h)) trl_ts_cg::launch_step(h->B, step, flags, lists, st);
     else trl_cg::launch_step(h->B, step, flags, lists, st);
 }
 static void terrain_launch(const trl_handle* h, cudaStream_t st) {
-    if (phys_slots(h)) trl_ps::launch_terrain(h->B, 0.5, st);
+    if (body_slots(h)) trl_bs::launch_terrain(h->B, 0.5, st);
+    else if (phys_slots(h)) trl_ps::launch_terrain(h->B, 0.5, st);
     else if (terrain_slots(h)) trl_ts::launch_terrain(h->B, 0.5, st);
     else launch_terrain(h->B, 0.5, st);
 }
 static void reset_launch(const trl_handle* h, const uint64_t* seeds, const int* env_ids, int count, int reseed) {
-    if (phys_slots(h)) trl_ps::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+    if (body_slots(h)) trl_bs::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
+    else if (phys_slots(h)) trl_ps::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
     else if (terrain_slots(h)) trl_ts::launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
     else launch_reset(h->B, seeds, env_ids, count, reseed, h->stream);
 }
@@ -705,6 +755,7 @@ trl_handle* trl_create(int argc, const char* const* argv, const char* data_root,
         delete h;
         return nullptr;
     }
+    h->data_root = data_root ? data_root : "";
     return trl_create_common(h, num_envs, device, mode, terrain_seeds, rng_seed);
 }
 
@@ -761,7 +812,8 @@ trl_handle* trl_create_common(trl_handle* h, int num_envs, int device, int mode,
     if (ensure_model(h)) return bail("upload_model failed");
     if (!ck(configure_step_kernels(), "configure_step_kernels") || !ck(trl_cg::configure_step_kernels(), "configure_step_kernels") ||
         !ck(trl_ts::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ts_cg::configure_step_kernels(), "configure_step_kernels") ||
-        !ck(trl_ps::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ps_cg::configure_step_kernels(), "configure_step_kernels"))
+        !ck(trl_ps::configure_step_kernels(), "configure_step_kernels") || !ck(trl_ps_cg::configure_step_kernels(), "configure_step_kernels") ||
+        !ck(trl_bs::configure_step_kernels(), "configure_step_kernels") || !ck(trl_bs_cg::configure_step_kernels(), "configure_step_kernels"))
         return bail("");
     if (!ck(configure_decide_kernel(), "configure_decide_kernel")) return bail("");
     if (!ck(configure_decide2_kernels(), "configure_decide2_kernels")) return bail("");
@@ -1552,11 +1604,12 @@ int trl_env_physics(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
 // a cell with any physics slot, or any cell of a handle whose envs are all on physics slot 0, is trl_eval_stats_cell's; the others come
 // from trl_phys_stats_kernel.  env_eval (trl_eval_stats_mode): only the envs whose present episode has mode `eval` (1 evaluates)
 static int eval_stats_phys(trl_handle* h, const std::string& who, int policy_slot, int terrain_slot, int phys_slot, const int* env_eval, int eval,
-                           int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+                           int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps, const int* env_body = nullptr,
+                           int body_slot = -1) {
     if (!h) return fail(who + ": null handle");
     if (phys_slot < -1 || phys_slot >= kMaxPhysSlots) return fail(who + ": physics slot " + std::to_string(phys_slot) + " out of range");
     if (phys_slot >= 0 && !phys_loaded(h, phys_slot)) return fail(who + ": physics slot " + std::to_string(phys_slot) + " is empty");
-    if (!env_eval && (phys_slot < 0 || !h->env_phys))
+    if (!env_eval && !env_body && (phys_slot < 0 || !h->env_phys))
         return eval_stats_cell(h, who.c_str(), policy_slot, terrain_slot, cycles, episodes, avg_dist, env_steps);
     if (policy_slot < -1 || policy_slot >= kMaxPolicySlots) return fail(who + ": policy slot " + std::to_string(policy_slot) + " out of range");
     if (policy_slot >= 0 && !slot_loaded(h, policy_slot)) return fail(who + ": policy slot " + std::to_string(policy_slot) + " is empty");
@@ -1565,7 +1618,8 @@ static int eval_stats_phys(trl_handle* h, const std::string& who, int policy_slo
     if (!h->phys_stats) CK(dalloc(h, &h->phys_stats, 4));
     double st[4];
     launch_phys_stats(h->B, h->slots_active ? h->P.env_slot : nullptr, h->env_phys, h->slots_active ? policy_slot : -1,
-                      h->env_terrain_host.empty() ? -1 : terrain_slot, h->env_phys ? phys_slot : -1, env_eval, eval, h->phys_stats, h->stream);
+                      h->env_terrain_host.empty() ? -1 : terrain_slot, h->env_phys ? phys_slot : -1, env_eval, eval, env_body, body_slot,
+                      h->phys_stats, h->stream);
     h->launches += 1;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(st, h->phys_stats, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
@@ -1640,16 +1694,16 @@ int trl_env_eval(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
 
 // trl_eval_stats_phys over the envs whose present episode runs in `mode`; a handle whose envs all run in one mode gives that mode
 // every env and the other none
-int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
-                        double* avg_dist, int64_t* env_steps) {
-    const std::string who = "trl_eval_stats_mode";
+// env_body (trl_eval_stats_body): only the envs whose present episode runs on body slot body_slot
+static int eval_stats_mode(trl_handle* h, const std::string& who, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles,
+                           int64_t* episodes, double* avg_dist, int64_t* env_steps, const int* env_body, int body_slot) {
     if (!h) return fail(who + ": null handle");
     if (mode != -1 && mode != TRL_MODE_POLI_EVAL && mode != TRL_MODE_EXPLORE)
         return fail(who + ": mode " + std::to_string(mode) + " is none of TRL_MODE_POLI_EVAL, TRL_MODE_EXPLORE or -1 (any)");
     if (mode == -1 || (!h->env_eval && mode == h->mode))
-        return eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, cycles, episodes, avg_dist, env_steps);
+        return eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, cycles, episodes, avg_dist, env_steps, env_body, body_slot);
     if (!h->env_eval) {     // no env runs in the other mode: the slots are checked, the figures are zero
-        if (eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, nullptr, nullptr, nullptr, nullptr)) return 1;
+        if (eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, nullptr, 0, nullptr, nullptr, nullptr, nullptr, env_body, body_slot)) return 1;
         if (cycles) *cycles = 0;
         if (episodes) *episodes = 0;
         if (avg_dist) *avg_dist = 0.0;
@@ -1657,7 +1711,169 @@ int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_sl
         return 0;
     }
     return eval_stats_phys(h, who, policy_slot, terrain_slot, phys_slot, h->env_eval, mode == TRL_MODE_POLI_EVAL ? 1 : 0, cycles, episodes,
-                           avg_dist, env_steps);
+                           avg_dist, env_steps, env_body, body_slot);
+}
+int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
+                        double* avg_dist, int64_t* env_steps) {
+    return eval_stats_mode(h, "trl_eval_stats_mode", mode, policy_slot, terrain_slot, phys_slot, cycles, episodes, avg_dist, env_steps, nullptr, -1);
+}
+
+static bool body_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxBodySlots && h->body_loaded[slot]); }
+
+// what every body of the table must satisfy (trl_load_body checks the file's numbers with its own messages; a checkpoint's table comes
+// through here only): finite numbers, positive masses and box sizes, gains and torque limits >= 0, reach within kMaxReach
+static bool body_ok(const BodyConst& b, int nj, std::string* why) {
+    auto finite = [&](const double* p, int k) { for (int i = 0; i < k; ++i) if (!std::isfinite(p[i])) return false; return true; };
+    for (const double* p : {b.attach_x, b.attach_y, b.mass, b.body_ax, b.body_ay, b.body_theta, b.body_cos, b.body_sin, b.half_x, b.half_y,
+                            b.izz_o, b.izz_c, b.kp, b.kd, b.torque_lim, b.target_theta0, b.target_vel})
+        if (!finite(p, nj)) { *why = "a per-link number is not finite"; return false; }
+    for (int j = 0; j < nj; ++j) {
+        if (b.has_limit[j] && !(std::isfinite(b.lim_lo[j]) && std::isfinite(b.lim_hi[j]))) { *why = "a joint limit is not finite"; return false; }
+        if (!(b.mass[j] > 0.0) || !(b.half_x[j] > 0.0) || !(b.half_y[j] > 0.0)) { *why = "a mass or box size is not positive"; return false; }
+        if (b.kp[j] < 0.0 || b.kd[j] < 0.0 || b.torque_lim[j] < 0.0) { *why = "Kp, Kd or TorqueLim is negative"; return false; }
+    }
+    if (!finite(b.corner_lx, 4 * nj) || !finite(b.corner_ly, 4 * nj) || !(b.total_mass > 0.0) || !(b.reach >= 0.0 && b.reach <= kMaxReach)) {
+        *why = "the corners, total mass or reach are out of range";
+        return false;
+    }
+    return true;
+}
+
+int trl_set_body_slot(trl_handle* h, int slot, const BodyConst& b) {
+    std::string why;
+    if (slot < 1 || slot >= kMaxBodySlots) return fail("body slot " + std::to_string(slot) + " out of range");
+    if (!body_ok(b, h->mc.nj, &why)) return fail("body slot " + std::to_string(slot) + ": " + why);
+    if (drain(h)) return 1;
+    if (!h->env_body) {     // first slot: from now on the step launches run the body-slot build
+        int* d = nullptr;
+        CK(dalloc(h, &d, 2 * (size_t)h->n));
+        h->env_body = d;
+        h->env_body_host.assign((size_t)h->n, 0);
+        destroy_graphs(h);
+    }
+    h->body[slot] = b;
+    h->body_loaded[slot] = true;
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail("trl_load_body: body table upload failed") : 0;
+}
+
+int trl_load_body(trl_handle* h, int slot, const char* character_json_path) {
+    const std::string who = "trl_load_body";
+    if (!h) return fail(who + ": null handle");
+    if (slot < 1 || slot >= kMaxBodySlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxBodySlots - 1) + "; slot 0 is the scene's body)");
+    if (!character_json_path) return fail(who + ": null path");
+    const ModelConst& sm = h->mc;
+    // the scene with this file's character records: fill_model derives from it what it derives for a handle created with
+    // -character_file=<this file>, and everything but the per-link numbers has to come out as the scene's
+    trl_handle t;
+    t.mode = h->mode;
+    try {
+        const CharacterRecords cr = read_character_file(join_path(h->data_root, character_json_path), h->data_root, sm.char_type == 2, sm.nj);
+        for (const char* rec : {"meta_f64", "pose0", "vel0", "terrain_params", "terrain_default_params", "net_out_scale"})
+            if (h->scene.has(rec)) t.scene.set_f64(rec, h->scene.f64(rec));
+        if (h->scene.has("net_dims")) t.scene.set_i32("net_dims", h->scene.i32("net_dims"));
+        std::vector<int32_t> mi = h->scene.i32("meta_i32");
+        if (mi.size() < 15) return fail(who + ": the scene's meta record is too short");
+        mi[8] = cr.nj; mi[9] = cr.ndof; mi[10] = cr.n_ctrl; mi[11] = cr.n_actions; mi[12] = cr.default_action; mi[13] = cr.grav_comp;
+        mi[14] = cr.virt_forces;
+        t.scene.set_i32("meta_i32", mi);
+        t.scene.set_f64("joints", cr.joints); t.scene.set_f64("bodies", cr.bodies); t.scene.set_f64("pd", cr.pd);
+        t.scene.set_f64("ctrl_params", cr.ctrl_params); t.scene.set_f64("actions", cr.actions);
+        const int nj = cr.nj;
+        for (int j = 0; j < nj; ++j) {
+            const double* r = &cr.joints[7 * j];
+            const double* b = &cr.bodies[9 * j];
+            const double* p = &cr.pd[6 * j];
+            const std::string at = " of link " + std::to_string(j);
+            for (int k : {2, 3, 5, 6})
+                if (!std::isfinite(r[k])) return fail(who + ": a Skeleton number" + at + " is not finite");
+            for (int k : {1, 2, 3, 5, 6, 7})
+                if (!std::isfinite(b[k])) return fail(who + ": a BodyDefs number" + at + " is not finite");
+            for (int k = 0; k < 5; ++k)
+                if (!std::isfinite(p[k])) return fail(who + ": a PDControllers number" + at + " is not finite");
+            if (!(b[1] > 0.0)) return fail(who + ": Mass" + at + " = " + std::to_string(b[1]) + " must be positive");
+            if (!(b[6] > 0.0) || !(b[7] > 0.0)) return fail(who + ": a box size" + at + " is not positive");
+            if (p[0] < 0.0 || p[1] < 0.0 || p[2] < 0.0) return fail(who + ": Kp, Kd or TorqueLim" + at + " is negative");
+        }
+    } catch (const std::exception& e) {
+        return fail(who + ": " + e.what());
+    }
+    if (fill_model(&t, sm.rng_seed)) return fail(who + ": the character's topology differs from the scene's: " + g_err);
+    const ModelConst& bm = t.mc;
+    // the topology, masks, corner layout, controller tables and net dimensions stay the scene's
+#define TRL_SAME(f) (std::memcmp(&bm.f, &sm.f, sizeof(sm.f)) == 0)
+    if (!(TRL_SAME(nj) && TRL_SAME(ndof) && TRL_SAME(parent) && TRL_SAME(dof) && TRL_SAME(collidable) && TRL_SAME(depth) &&
+          TRL_SAME(max_depth) && TRL_SAME(child) && TRL_SAME(anc_pow) && TRL_SAME(n_chains) && TRL_SAME(chain_levels) &&
+          TRL_SAME(chain_level_len) && TRL_SAME(chain_links) && TRL_SAME(chain_len) && TRL_SAME(chain_level) && TRL_SAME(chain_merge) &&
+          TRL_SAME(chain_up) && TRL_SAME(n_corners) && TRL_SAME(corner_base) && TRL_SAME(anc_mask_toe) && TRL_SAME(anc_mask_finger) &&
+          TRL_SAME(vf_mask_toe) && TRL_SAME(vf_mask_finger)))
+        return fail(who + ": the character's topology (joint types, parents or body shapes) differs from the scene's");
+    if (!(TRL_SAME(n_ctrl) && TRL_SAME(n_actions) && TRL_SAME(default_action) && TRL_SAME(grav_comp) && TRL_SAME(virt_forces) &&
+          TRL_SAME(ctrl_params) && TRL_SAME(act_idx0) && TRL_SAME(act_idx1) && TRL_SAME(act_cyclic) && TRL_SAME(act_blend)))
+        return fail(who + ": the character's Controllers section (controller files, actions, default action or flags) differs from the scene's");
+#undef TRL_SAME
+    if (bm.reach > kMaxReach)
+        return fail(who + ": the body reaches " + std::to_string(bm.reach) + " m from its root joint, more than the " + std::to_string(kMaxReach) +
+                    " m the ground window covers (UpdateGround keeps 2 m behind the root; the broad phase reads reach + 0.25 m)");
+    if (drain(h)) return 1;
+    if (h->env_body) {
+        std::vector<int> cur((size_t)h->n);
+        CK(cudaMemcpy(cur.data(), h->env_body, cur.size() * 4, cudaMemcpyDeviceToHost));
+        for (int e = 0; e < h->n; ++e)
+            if (cur[e] == slot || h->env_body_host[e] == slot)
+                return fail(who + ": slot " + std::to_string(slot) + " is in use (env " + std::to_string(e) + "'s present or assigned body)");
+    }
+    return trl_set_body_slot(h, slot, body_of(bm));
+}
+
+int trl_set_env_body(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
+    const std::string who = "trl_set_env_body";
+    if (!h) return fail(who + ": null handle");
+    if (n < 0 || n > h->n) return fail(who + ": env count out of range");
+    if (n > 0 && !slots) return fail(who + ": null slot list");
+    for (int k = 0; k < n; ++k) {
+        const int e = env_ids ? env_ids[k] : k;
+        if (e < 0 || e >= h->n) return fail(who + ": env id " + std::to_string(e) + " out of range");
+        if (slots[k] < 0 || slots[k] >= kMaxBodySlots) return fail(who + ": slot " + std::to_string(slots[k]) + " out of range");
+        if (!body_loaded(h, slots[k])) return fail(who + ": slot " + std::to_string(slots[k]) + " is empty (trl_load_body first)");
+    }
+    if (!h->env_body) return 0;      // only slot 0 exists, and every env is on it
+    std::vector<int> next = h->env_body_host;
+    for (int k = 0; k < n; ++k) next[env_ids ? env_ids[k] : k] = slots[k];
+    if (drain(h)) return 1;
+    CK(cudaMemcpy(h->env_body + h->n, next.data(), next.size() * 4, cudaMemcpyHostToDevice));
+    h->env_body_host.swap(next);
+    return 0;
+}
+
+int trl_env_body(trl_handle* h, int32_t* current, int32_t* assigned, int n) {
+    if (!h) return fail("trl_env_body: null handle");
+    if (n < 0 || n > h->n) return fail("trl_env_body: env count out of range");
+    if (!h->env_body) {
+        for (int k = 0; k < n; ++k) {
+            if (current) current[k] = 0;
+            if (assigned) assigned[k] = 0;
+        }
+        return 0;
+    }
+    if (drain(h)) return 1;
+    if (current && n > 0) CK(cudaMemcpy(current, h->env_body, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (assigned && n > 0) CK(cudaMemcpy(assigned, h->env_body + h->n, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+// trl_eval_stats_mode over the envs whose present episode runs on body slot body_slot (-1: any); a handle whose envs are all on body
+// slot 0 needs no filter
+int trl_eval_stats_body(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int body_slot, int64_t* cycles,
+                        int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+    const std::string who = "trl_eval_stats_body";
+    if (!h) return fail(who + ": null handle");
+    if (body_slot < -1 || body_slot >= kMaxBodySlots) return fail(who + ": body slot " + std::to_string(body_slot) + " out of range");
+    if (body_slot >= 0 && !body_loaded(h, body_slot)) return fail(who + ": body slot " + std::to_string(body_slot) + " is empty");
+    const bool filter = body_slot >= 0 && h->env_body;
+    return eval_stats_mode(h, who, mode, policy_slot, terrain_slot, phys_slot, cycles, episodes, avg_dist, env_steps, filter ? h->env_body : nullptr,
+                           filter ? body_slot : -1);
 }
 
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {

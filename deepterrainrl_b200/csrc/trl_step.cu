@@ -44,7 +44,14 @@
 // Physics slots (trl_load_physics) are served by a third pair, trl_step_ps.cu (namespace trl_ps) and trl_step_ps_cg.cu (trl_ps_cg),
 // compiled with TRL_PHYS_SLOTS_VARIANT as well as TRL_TERRAIN_SLOTS_VARIANT: their physics sub-steps read the env's own slot of
 // c_phys.  The emulator's "always with slots" includes physics slots; a handle without any has no per-env array and reads slot 0.
-#if defined(TRL_PHYS_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
+// Body slots (trl_load_body) are served by a fourth pair, trl_step_bs.cu (namespace trl_bs) and trl_step_bs_cg.cu (trl_bs_cg), compiled
+// with TRL_BODY_SLOTS_VARIANT as well as the terrain- and physics-slot flags: every warp stages the link and box tables of its own
+// env's body, and the per-link reads of the controller take the env's slot of g_body.  The emulator includes body slots too.
+#if defined(TRL_BODY_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
+#define TRL_IMPL_NS trl_bs_cg
+#elif defined(TRL_BODY_SLOTS_VARIANT)
+#define TRL_IMPL_NS trl_bs
+#elif defined(TRL_PHYS_SLOTS_VARIANT) && defined(TRL_CG_VARIANT)
 #define TRL_IMPL_NS trl_ps_cg
 #elif defined(TRL_PHYS_SLOTS_VARIANT)
 #define TRL_IMPL_NS trl_ps
@@ -101,6 +108,37 @@ __device__ ModelConst g_model;
 #else
 #define LT(field, idx) c_model.field[(idx)]
 #define LT2(field, i, j) c_model.field[(i)][(j)]
+#endif
+#ifndef TRL_LINK_SMEM
+#define TRL_LINK_SMEM 1     // 1: the per-lane link constants live in shared memory (one table per CTA) instead of ~28 registers per thread
+                            //    (the register build spills them and reloads them inside the ABA rounds)
+#endif
+// Body slots: the per-link numbers of the env's body.  `bs` (the env's slot, warp-uniform: one env per warp) must be in scope.
+// BL: lane-indexed reads from the mirror g_body at the slot's base; BU: warp-uniform reads of a per-link number; BM: the slot's
+// total_mass / reach from constant memory (one broadcast).  The other builds read the scene's body from the model, as before slots.
+// The body build needs the link tables in shared memory (restaged per warp when its env changes body); the emulator's
+// TRL_LINK_SMEM=0 experiment build runs without body slots.
+#if (defined(TRL_BODY_SLOTS_VARIANT) || defined(TRL_SIMT_EMU)) && TRL_LINK_SMEM
+#define TRL_BODY_TABLE 1
+__device__ BodyConst g_body[kMaxBodySlots];      // slot 0 = the scene's body (trl_types.h: BodyConst)
+__constant__ double c_body_total_mass[kMaxBodySlots], c_body_reach[kMaxBodySlots];   // total_mass, reach of every slot
+__constant__ int* c_env_body;                    // [2][n] of the owning handle: the body slot of every env's present episode, then the slot
+                                                 // it gets at its next reset; null while the handle has no body slot
+#define BL(field, idx) __ldg(&g_body[bs].field[(idx)])
+#define BU(field, idx) BL(field, idx)
+#define BM(field) c_body_##field[bs]
+#define TRL_BS_DECL , int bs
+#define TRL_BS_ARG , bs
+#else
+#if defined(TRL_BODY_SLOTS_VARIANT)
+#error "the body-slot build stages its link tables in shared memory (TRL_LINK_SMEM=1)"
+#endif
+#define TRL_BODY_TABLE 0
+#define BL(field, idx) LT(field, idx)
+#define BU(field, idx) c_model.field[(idx)]
+#define BM(field) c_model.field
+#define TRL_BS_DECL
+#define TRL_BS_ARG
 #endif
 
 #ifndef TRL_WARPS_PER_BLOCK
@@ -461,11 +499,7 @@ __device__ void store_rng(Lane& L, const CounterRng& r) {
 }
 
 // ================================================================================================ warp context
-// Per-lane constants of link `lane` and the env state held in registers.
-#ifndef TRL_LINK_SMEM
-#define TRL_LINK_SMEM 1     // 1: the per-lane link constants live in shared memory (one table per CTA) instead of ~28 registers per thread
-                            //    (the register build spills them and reloads them inside the ABA rounds)
-#endif
+// Per-lane constants of link `lane` and the env state held in registers (TRL_LINK_SMEM: above).
 #if TRL_LINK_SMEM
 enum { LF_AX, LF_AY, LF_MASS, LF_BAX, LF_BAY, LF_IZZ, LF_LIM_LO, LF_LIM_HI, LF_NUM };
 enum { LI_PARENT, LI_DEPTH, LI_ANC1, LI_ANC2, LI_ANC4, LI_ANC8, LI_CH_LEN, LI_CH_LEVEL, LI_CH_MERGE, LI_CH_UP, LI_NUM };
@@ -518,7 +552,7 @@ struct LinkVals {
     unsigned long long ch_links;
     double ax, ay, mass, bax, bay, izz_c, lim_lo, lim_hi;
 };
-__device__ __forceinline__ LinkVals link_values(int lane) {
+__device__ __forceinline__ LinkVals link_values(int lane TRL_BS_DECL) {
     const ModelConst& m = c_model;
     LinkVals c;
     c.act = lane < m.nj;
@@ -538,21 +572,28 @@ __device__ __forceinline__ LinkVals link_values(int lane) {
     if (c.anc2 < 0) c.anc2 = kZeroLane;
     if (c.anc4 < 0) c.anc4 = kZeroLane;
     if (c.anc8 < 0) c.anc8 = kZeroLane;
-    c.ax = LT(attach_x, j); c.ay = LT(attach_y, j);
-    c.mass = c.act ? LT(mass, j) : 0.0;
-    c.bax = LT(body_ax, j); c.bay = LT(body_ay, j);
-    c.izz_c = c.act ? LT(izz_c, j) : 0.0;
-    const int has_lim = c.act ? LT(has_limit, j) : 0;
-    c.lim_lo = has_lim ? LT(lim_lo, j) : -INFINITY;    // no limit: never violated, so the limit force needs no branch
-    c.lim_hi = has_lim ? LT(lim_hi, j) : INFINITY;
+    c.ax = BL(attach_x, j); c.ay = BL(attach_y, j);
+    c.mass = c.act ? BL(mass, j) : 0.0;
+    c.bax = BL(body_ax, j); c.bay = BL(body_ay, j);
+    c.izz_c = c.act ? BL(izz_c, j) : 0.0;
+    const int has_lim = c.act ? BL(has_limit, j) : 0;
+    c.lim_lo = has_lim ? BL(lim_lo, j) : -INFINITY;    // no limit: never violated, so the limit force needs no branch
+    c.lim_hi = has_lim ? BL(lim_hi, j) : INFINITY;
     return c;
 }
-// TRL_LINK_SMEM: the first warp of the CTA fills the table (the caller's __syncthreads() publishes it)
-__device__ __forceinline__ void stage_link_tables(LinkTables* t) {
+// TRL_LINK_SMEM: the first warp of the CTA fills the table (the caller's __syncthreads() publishes it); in the body build every warp
+// fills its own table with the links of body slot bs (the caller's __syncwarp() publishes it)
+__device__ __forceinline__ void stage_link_tables(LinkTables* t TRL_BS_DECL) {
 #if TRL_LINK_SMEM
+#if TRL_BODY_TABLE
+    {
+        const int lane = threadIdx.x & 31;
+        const LinkVals v = link_values(lane, bs);
+#else
     if (threadIdx.x < kWarp) {
         const int lane = threadIdx.x;
         const LinkVals v = link_values(lane);
+#endif
         t->d[LF_AX * kWarp + lane] = v.ax; t->d[LF_AY * kWarp + lane] = v.ay; t->d[LF_MASS * kWarp + lane] = v.mass;
         t->d[LF_BAX * kWarp + lane] = v.bax; t->d[LF_BAY * kWarp + lane] = v.bay; t->d[LF_IZZ * kWarp + lane] = v.izz_c;
         t->d[LF_LIM_LO * kWarp + lane] = v.lim_lo; t->d[LF_LIM_HI * kWarp + lane] = v.lim_hi;
@@ -587,6 +628,37 @@ __device__ __forceinline__ LinkC load_link(int lane, const LinkTables* t) {
 #endif
     return c;
 }
+#if TRL_BODY_TABLE
+// The warp's own tables for body slot bs: the link table, and (s_clx non-null) the corner tables with the six per-body box tables behind
+// them (the layout the other builds stage once per CTA in trl_step_kernel).  The leading barrier lets every lane finish reading the tables
+// of the env's previous body; the trailing one publishes the new ones.
+__device__ __forceinline__ void stage_body(LinkTables* lt, double* s_clx, double* s_cly, int lane, int bs) {
+    const ModelConst& m = c_model;
+    __syncwarp();
+    stage_link_tables(lt, bs);
+    if (s_clx) {
+        for (int t = lane; t < m.n_corners; t += kWarp) { s_clx[t] = BL(corner_lx, t); s_cly[t] = BL(corner_ly, t); }
+        if (lane < m.nj) {
+            double* tb = s_clx + 4 * kMaxJoints;
+            const int t = lane;
+            tb[t] = BL(body_ax, t); tb[kMaxJoints + t] = BL(body_ay, t); tb[2 * kMaxJoints + t] = BL(body_cos, t); tb[3 * kMaxJoints + t] = BL(body_sin, t);
+            tb[4 * kMaxJoints + t] = BL(half_x, t); tb[5 * kMaxJoints + t] = BL(half_y, t);
+        }
+    }
+    __syncwarp();
+}
+// at an episode reset: the body slot assigned to the env (trl_set_env_body) becomes its current one, and the warp restages its tables
+// for it.  Returns the slot
+__device__ __forceinline__ int begin_body(const Lane& L, LinkTables* lt, double* s_clx, double* s_cly, int lane) {
+    int bs = 0;
+    if (c_env_body) {
+        bs = c_env_body[(size_t)L.n + L.env];
+        if (lane == 0) c_env_body[L.env] = bs;
+    }
+    stage_body(lt, s_clx, s_cly, lane, bs);
+    return bs;
+}
+#endif
 
 // root-ward prefix sums over the kinematic tree by pointer jumping: after 4 rounds every link holds the sum of its own
 // value and those of all its ancestors (depth <= 15), using the static 2^k-th ancestor table.  A missing ancestor points
@@ -810,7 +882,7 @@ __device__ __forceinline__ void chain_aba(double* xs, const ChainC& ch, int lane
 // ================================================================================================ controller half
 // Returns the clamped joint torque of link `lane` (0 for the root and idle lanes).
 __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, const Kin& k, double* xs, int lane,
-                                    double h, int contact) {
+                                    double h, int contact TRL_BS_DECL) {
     const double lk_mass = lc.mass;      // read once (shared-memory table; a read cannot move across the shuffles below)
     const ModelConst& m = c_model;
     const int md = m.max_depth;
@@ -869,9 +941,9 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
     const bool active_vf = raptor && (state == rsContact || state == rsDown) && ((contact >> st_toe) & 1);
     {
         double bvx = lk_mass * (k.vx - k.w * k.cy);
-        double comvx = warp_sum_all(bvx) / m.total_mass;
+        double comvx = warp_sum_all(bvx) / BM(total_mass);
         if (raptor) {
-            double comx = warp_sum_all(lk_mass * k.cx) / m.total_mass;
+            double comx = warp_sum_all(lk_mass * k.cx) / BM(total_mass);
             double toe_x = shf(k.cx, st_toe);
             if (lane == 0) {
                 bool first_half = state == rsContact || state == rsDown;
@@ -894,18 +966,18 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
     double tau0 = 0.0, rhs_link = 0.0, kd_link = 0.0, kd_eff = 0.0;
     if (lc.act && lane > 0) {
         double theta = e.q;
-        if (LT(world_pd, lane)) {
+        if (BL(world_pd, lane)) {
             // child body's world rotation, wrapped (cPDController::CalcTheta, sim/PDController.cpp:181-198)
-            double c = k.cw * LT(body_cos, lane) - k.sw * LT(body_sin, lane);
-            double s = k.sw * LT(body_cos, lane) + k.cw * LT(body_sin, lane);
+            double c = k.cw * BL(body_cos, lane) - k.sw * BL(body_sin, lane);
+            double s = k.sw * BL(body_cos, lane) + k.cw * BL(body_sin, lane);
             double a = acos(fmin(1.0, fmax(-1.0, c)));
             theta = (s >= 0) ? a : -a;
         }
         const bool pd_on = !(active_vf && lane == st_hip);
-        kd_link = LT(kd, lane);
+        kd_link = BL(kd, lane);
         kd_eff = pd_on ? kd_link : 0.0;
-        double perr = L.d(D_PD_TARGET + lane) - theta, verr = LT(target_vel, lane) - e.qd;
-        tau0 = pd_on ? (LT(kp, lane) * (perr - h * e.qd) + kd_link * verr) : 0.0;
+        double perr = L.d(D_PD_TARGET + lane) - theta, verr = BL(target_vel, lane) - e.qd;
+        tau0 = pd_on ? (BL(kp, lane) * (perr - h * e.qd) + kd_link * verr) : 0.0;
         rhs_link = tau0 - Cj;
     }
     // (M + h Kd) acc = rhs is the articulated-body problem of the same tree at rest: no velocity products, no gravity, joint
@@ -939,10 +1011,10 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
     // foot bottom-centre positions (GetEndEffectorContactPos), relative to O
     double ex[2], ey[2];
     {
-        double bc = k.cw * LT(body_cos, lc.act ? lane : 0) - k.sw * LT(body_sin, lc.act ? lane : 0);
-        double bs = k.sw * LT(body_cos, lc.act ? lane : 0) + k.cw * LT(body_sin, lc.act ? lane : 0);
-        double ly = -LT(half_y, lc.act ? lane : 0);
-        double px = k.cx - bs * ly, py = k.cy + bc * ly;
+        double bc = k.cw * BL(body_cos, lc.act ? lane : 0) - k.sw * BL(body_sin, lc.act ? lane : 0);
+        double bsn = k.sw * BL(body_cos, lc.act ? lane : 0) + k.cw * BL(body_sin, lc.act ? lane : 0);
+        double ly = -BL(half_y, lc.act ? lane : 0);
+        double px = k.cx - bsn * ly, py = k.cy + bc * ly;
         ex[0] = shf(px, eff0); ey[0] = shf(py, eff0);
         ex[1] = shf(px, eff1); ey[1] = shf(py, eff1);
     }
@@ -1014,7 +1086,7 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
         const double sw_tau = shf(tau, sw_hip), th0 = shf(e.q, 0), thd0 = shf(e.qd, 0);
         if (active_vf && lane == st_hip) {
             int base = D_PARAMS + m.misc_max + state * m.sp_max;
-            double root_tau = m.kp[st_hip] * (L.d(base + rpRootPitch) - wrap_pi(th0)) + m.kd[st_hip] * (-thd0);
+            double root_tau = BU(kp, st_hip) * (L.d(base + rpRootPitch) - wrap_pi(th0)) + BU(kd, st_hip) * (-thd0);
             tau += -sw_tau - root_tau;
         }
     }
@@ -1045,7 +1117,7 @@ __device__ double controller_torque(Lane& L, const LinkC& lc, const EnvRegs& e, 
 
     // ---- cJoint::ApplyTorque clamp (sim/Joint.cpp:171-201,257-264)
     if (lc.act && lane > 0) {
-        double lim = LT(torque_lim, lane);
+        double lim = BL(torque_lim, lane);
         if (fabs(tau) > lim) tau *= lim / fabs(tau);
     } else tau = 0.0;
     TRL_CLK_END(PH_CTRL_REST, clk);
@@ -1252,15 +1324,20 @@ __device__ void build_poli_state(const LinkC& lc, const EnvRegs& e, const Kin& k
 
 // cScenarioSimChar::Reset (+ PoliEval / Exp specifics): scenarios/ScenarioSimChar.cpp:121-132.  Cooperative kinematics,
 // scalar bookkeeping + terrain generation on lane 0.
-__device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B, int lane TRL_RESET_XS_DECL) {
+__device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B, int lane TRL_RESET_XS_DECL TRL_BS_DECL) {
     const ModelConst& m = c_model;
+#if TRL_BODY_TABLE
+    // the PD targets no gait state sets keep the TargetTheta of the episode's body (the others are set by apply_action below)
+    if (lc.act) L.d(D_PD_TARGET + lane) = BL(target_theta0, lane);
+    __syncwarp();
+#endif
     e.q = lc.act ? m.pose0[lane == 0 ? 2 : lane + 2] : 0.0;
     e.qd = lc.act ? m.vel0[lane == 0 ? 2 : lane + 2] : 0.0;
     e.ox = m.pose0[0]; e.oy = m.pose0[1]; e.oxd = m.vel0[0]; e.oyd = m.vel0[1];
     e.tau = 0.0;
     Kin k = kinematics(lc, e TRL_KIN_XS_ARG);
-    double comx = e.ox + warp_sum_all(lc.mass * k.cx) / m.total_mass;
-    double comy = e.oy + warp_sum_all(lc.mass * k.cy) / m.total_mass;
+    double comx = e.ox + warp_sum_all(lc.mass * k.cx) / BM(total_mass);
+    double comy = e.oy + warp_sum_all(lc.mass * k.cy) / BM(total_mass);
     double newx = e.ox, newy = e.oy;
     if (lane == 0) {
         L.i(I_CONTACT) = 0;
@@ -1345,10 +1422,17 @@ __device__ __forceinline__ void catchup_leave(const Buffers& B, int prev) {
 
 __global__ void __launch_bounds__(kBlockThreads, TRL_STEP_MIN_BLOCKS)
 trl_step_kernel(Buffers B, double h, int flags, int lists) {
+#if TRL_BODY_TABLE
+    // one copy of the link, corner and box tables per warp, staged below with its env's body
+    __shared__ double s_clx_w[kWarpsPerBlock][4 * kMaxJoints + 6 * kMaxJoints], s_cly_w[kWarpsPerBlock][4 * kMaxJoints];
+    __shared__ LinkTables s_link_w[kWarpsPerBlock];
+#else
     __shared__ double s_clx[4 * kMaxJoints + 6 * kMaxJoints], s_cly[4 * kMaxJoints];     // s_clx also carries the six per-body box tables
+#endif
     __shared__ __align__(16) double s_x[kWarpsPerBlock * X_END];
     TRL_CLK_BEGIN(clk);
     const ModelConst& m = c_model;
+#if !TRL_BODY_TABLE
     for (int t = threadIdx.x; t < m.n_corners; t += kBlockThreads) {
         s_clx[t] = LT(corner_lx, t); s_cly[t] = LT(corner_ly, t);
     }
@@ -1358,14 +1442,22 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         tb[4 * kMaxJoints + t] = LT(half_x, t); tb[5 * kMaxJoints + t] = LT(half_y, t);
     }
     TRL_LINK_TABLES_DECL
+#endif
 #if TRL_FIELD_SMEM
     static_assert(I_NUM_FIELDS <= kWarp, "one lane per i32 field");
     __shared__ double s_fd[kWarpsPerBlock * D_NUM_FIELDS];
     __shared__ int s_fi[kWarpsPerBlock * I_NUM_FIELDS];
 #endif
+#if !TRL_BODY_TABLE
     stage_link_tables(link_tabs);
     __syncthreads();
+#endif
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#if TRL_BODY_TABLE
+    double* const s_clx = s_clx_w[warp];
+    double* const s_cly = s_cly_w[warp];
+    LinkTables* const link_tabs = &s_link_w[warp];
+#endif
     // pending-decision lists (lag + 1 of them, used round robin by successive env-steps): envs that reach a cycle boundary in this
     // launch are appended to list `app`; an env's I_PENDING tag is 1 + the list it was last appended to.  The decision of a list is
     // made on a side stream and its envs are then caught up over `lag` env-steps by a side launch (trl_host.cu: enqueue_update), so
@@ -1418,6 +1510,10 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         L.i(I_PENDING) = 0;    // serial schedule / end of the update: every decision has been served before this launch
     }
     double* xs = s_x + warp * X_END;
+#if TRL_BODY_TABLE
+    int bs = c_env_body ? c_env_body[env] : 0;    // the body of the env's present episode; an episode reset below may change it
+    stage_body(link_tabs, s_clx, s_cly, lane, bs);
+#endif
     const LinkC lc = load_link(lane, link_tabs);
     EnvRegs e;
     load_env(L, lc, e, lane);
@@ -1441,7 +1537,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         k_ctrl = k; have_k = true;
 #endif
         TRL_CLK_END(PH_KIN, clk);
-        e.tau = controller_torque(L, lc, e, k, xs, lane, h, contact);
+        e.tau = controller_torque(L, lc, e, k, xs, lane, h, contact TRL_BS_ARG);
         TRL_CLK_RESET(clk);
         if (lane == 0) {
             // fall checks (sim/SimCharSoftFall.cpp:74-125)
@@ -1497,7 +1593,10 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
             do_reset = true;
         }
         if (do_reset) {
-            reset_env(L, lc, e, B, lane TRL_RESET_XS_ARG); contact = 0;
+#if TRL_BODY_TABLE
+            bs = begin_body(L, link_tabs, s_clx, s_cly, lane);   // lc reads the warp's tables, which now hold the new episode's body
+#endif
+            reset_env(L, lc, e, B, lane TRL_RESET_XS_ARG TRL_BS_ARG); contact = 0;
 #if TRL_REUSE_KIN
             have_k = false;
 #endif
@@ -1515,7 +1614,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         const double dt = h / ns;
         // terrain maximum over the window the character's corners can reach during this env-step; kClearMargin covers the
         // contact tolerance measured along the surface normal on (near-)vertical cliff faces and the root's travel
-        const double clear_y = g.window_max(e.ox - m.reach - 0.25, e.ox + m.reach + 0.25, lane) + kClearMargin;
+        const double clear_y = g.window_max(e.ox - BM(reach) - 0.25, e.ox + BM(reach) + 0.25, lane) + kClearMargin;
 #if TRL_PHYS_TABLE
         // the slot of the env's present episode (a reset above has already made its assignment current)
         const int ps = c_env_phys ? c_env_phys[env] : 0;
@@ -1580,8 +1679,8 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
             // cycle boundary: build the policy state and hand the env to the decision kernel
             Kin k = kinematics(lc, e TRL_KIN_XS_ARG);
             build_poli_state(lc, e, k, B, g, env, lane, TRL_IS_RAPTOR(m) ? L.i(I_STANCE) : 0);
-            double comx = e.ox + warp_sum_all(lc.mass * k.cx) / m.total_mass;
-            double comy = e.oy + warp_sum_all(lc.mass * k.cy) / m.total_mass;
+            double comx = e.ox + warp_sum_all(lc.mass * k.cx) / BM(total_mass);
+            double comy = e.oy + warp_sum_all(lc.mass * k.cy) / BM(total_mass);
             if (lane == 0) {
                 B.com_stash[env] = comx; B.com_stash[B.n + env] = comy;
                 L.i(I_FIRST_CYCLE) = 0;
@@ -1611,10 +1710,15 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
 // Initial reset of every env (trl_create / trl_reset): seeds the terrain RNG and runs the episode reset.
 __global__ void __launch_bounds__(kBlockThreads)
 trl_reset_kernel(Buffers B, const uint64_t* terrain_seeds, const int* env_ids, int count, int reseed) {
+#if TRL_BODY_TABLE
+    __shared__ LinkTables s_link_w[kWarpsPerBlock];     // staged per warp with the body of the episode the reset starts (below)
+    LinkTables* const link_tabs = &s_link_w[threadIdx.x >> 5];
+#else
     TRL_LINK_TABLES_DECL
 #if TRL_LINK_SMEM
     stage_link_tables(link_tabs);
     __syncthreads();
+#endif
 #endif
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int idx = blockIdx.x * kWarpsPerBlock + warp;
@@ -1634,13 +1738,16 @@ trl_reset_kernel(Buffers B, const uint64_t* terrain_seeds, const int* env_ids, i
         L.d(D_CUR_CYCLE_T) = 0.0; L.d(D_CUR_STUMBLE) = 0.0; L.d(D_PREV_COM_X) = 0.0; L.d(D_PREV_COM_Y) = 0.0;
     }
     __syncwarp();
+#if TRL_BODY_TABLE
+    const int bs = begin_body(L, link_tabs, nullptr, nullptr, lane);
+#endif
     const LinkC lc = load_link(lane, link_tabs);
     EnvRegs e;
 #if TRL_KIN_SMEM
     __shared__ __align__(16) double s_pfx[kWarpsPerBlock * 3 * 2 * kWarp];
     double* xs = s_pfx + warp * 3 * 2 * kWarp - X_PFX;    // kinematics() only touches [X_PFX, X_PFX_END)
 #endif
-    reset_env(L, lc, e, B, lane TRL_RESET_XS_ARG);
+    reset_env(L, lc, e, B, lane TRL_RESET_XS_ARG TRL_BS_ARG);
     store_env(L, lc, e, lane);
 }
 
@@ -1717,6 +1824,21 @@ cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval) {
     return e;
 }
 #endif
+#if TRL_BODY_TABLE
+// the body table (slot 0 = the scene's body) and the handle's per-env slot array (null: every env on slot 0), uploaded with the model
+cudaError_t upload_body(const BodyConst* body, int* env_body) {
+    double tm[kMaxBodySlots], rc[kMaxBodySlots];
+    for (int s = 0; s < kMaxBodySlots; ++s) { tm[s] = body[s].total_mass; rc[s] = body[s].reach; }
+    cudaError_t e = cudaMemcpyToSymbol(g_body, body, sizeof(BodyConst) * kMaxBodySlots);
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_body_total_mass, tm, sizeof(tm));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_body_reach, rc, sizeof(rc));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_body, &env_body, sizeof(env_body));
+    return e;
+}
+#elif defined(TRL_SIMT_EMU)
+// the emulator's TRL_LINK_SMEM=0 experiment build has no body slots: a handle with one is refused
+cudaError_t upload_body(const BodyConst*, int* env_body) { return env_body ? static_cast<cudaError_t>(1) : cudaSuccess; }
+#endif
 size_t step_smem_bytes() { return 0; }
 // TRL_PHASE_CLOCKS builds: copy the accumulated phase clocks (kNumPhases + the env-step count) into out[], optionally zero them
 cudaError_t step_phase_clocks(unsigned long long* out, int reset) {
@@ -1764,7 +1886,7 @@ void launch_reset(const Buffers& B, const uint64_t* seeds, const int* env_ids, i
 
 }  // namespace TRL_IMPL_NS
 
-#if !defined(TRL_CG_VARIANT) && !defined(TRL_TERRAIN_SLOTS_VARIANT) && !defined(TRL_PHYS_SLOTS_VARIANT)
+#if !defined(TRL_CG_VARIANT) && !defined(TRL_TERRAIN_SLOTS_VARIANT) && !defined(TRL_PHYS_SLOTS_VARIANT) && !defined(TRL_BODY_SLOTS_VARIANT)
 #include "trl_decide.cuh"
 #include "trl_decide2.cuh"
 #endif

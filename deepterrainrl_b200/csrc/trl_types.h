@@ -169,6 +169,29 @@ constexpr int kMaxPhysSlots = 8;
 constexpr double kClearMargin = 0.05;
 constexpr double kMaxSlope = 25.0;
 
+// Body slots: slot 0 is the scene's own body (the per-link numbers of ModelConst), slots 1 .. kMaxBodySlots - 1 are loaded from
+// character files of the scene's topology and controllers by trl_load_body.  A slot holds every per-link number fill_model reads from a
+// character file, and what it derives from them; the topology, masks, corner layout, controller tables and net dimensions stay
+// ModelConst's.  The body-slot build of the env-step kernels reads the table from a global-memory mirror (lane-indexed reads) and
+// total_mass / reach from a __constant__ copy (warp-uniform reads); the per-env slots ([2][n]: current, assigned) are an allocation of
+// their own, so ModelConst, Buffers and the planes keep their layout.
+constexpr int kMaxBodySlots = 8;
+struct BodyConst {
+    double attach_x[kMaxJoints], attach_y[kMaxJoints], lim_lo[kMaxJoints], lim_hi[kMaxJoints];
+    int has_limit[kMaxJoints];
+    double mass[kMaxJoints], body_ax[kMaxJoints], body_ay[kMaxJoints], body_theta[kMaxJoints], body_cos[kMaxJoints], body_sin[kMaxJoints];
+    double half_x[kMaxJoints], half_y[kMaxJoints], izz_o[kMaxJoints], izz_c[kMaxJoints];
+    double corner_lx[4 * kMaxJoints], corner_ly[4 * kMaxJoints];
+    double kp[kMaxJoints], kd[kMaxJoints], torque_lim[kMaxJoints], target_theta0[kMaxJoints], target_vel[kMaxJoints];
+    int world_pd[kMaxJoints];
+    double total_mass, reach;
+};
+// The broad phase of the env-step reads the terrain maximum over [x - reach - 0.25, x + reach + 0.25] around the root joint
+// (trl_step.cu: window_max).  That window has to lie inside the ground the env holds: UpdateGround keeps [x - 2, x + 11] generated,
+// so the body of a slot may reach at most kMaxReach = 2 - 0.25 m behind the root (the front side has 11 m).  The shipped characters
+// reach about 1.1 m (dog, goat) and 1.0 m (raptor); trl_load_body refuses a reach above kMaxReach.
+constexpr double kMaxReach = 1.75;
+
 // Exploration settings can change between updates (cScenarioExp::SetExpRate/Temp/BaseActionRate).
 struct ExpSettings {
     int enable;

@@ -46,6 +46,8 @@ VARIANTS = {
     "smem_xchg_decide_tile4": ["-DTRL_SMEM_XCHG=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
     "all": ["-DTRL_SMEM_XCHG=1", "-DTRL_REUSE_KIN=1", "-DTRL_DECIDE_TILE=1", "-DTRL_CONV_TILE=4"],
 }
+# The body-slot units (trl_step_bs.cu, trl_step_bs_cg.cu) are not among them: a variant library links the product's body-slot objects,
+# since their per-warp tables need TRL_LINK_SMEM=1 and fit the 48 KB of static shared memory only at the product's 4 warps per CTA.
 STEP_UNITS = ("trl_step.cu", "trl_step_cg.cu", "trl_step_ts.cu", "trl_step_ts_cg.cu", "trl_step_ps.cu", "trl_step_ps_cg.cu")      # the only translation units the variant flags reach
 
 
@@ -72,9 +74,9 @@ def build_library(force=False, verbose=False):
     """Compile csrc/*.cu for sm_90a into lib/libterrainrl_b200.so (nvcc cross-compiles without a GPU).
     trl_step_cg.cu is the env-step translation unit again with -Xptxas -dlcm=cg (L1-bypassing loads, see trl_step.cu);
     trl_step_ts.cu / trl_step_ts_cg.cu are both again with terrain slots, trl_step_ps.cu / trl_step_ps_cg.cu with terrain and
-    physics slots.
-    With TRL_VARIANT set, the two env-step units are compiled with the variant's flags and linked with the product's other
-    objects into lib/variants/<name>/."""
+    physics slots, trl_step_bs.cu / trl_step_bs_cg.cu with terrain, physics and body slots.
+    With TRL_VARIANT set, the env-step units of STEP_UNITS are compiled with the variant's flags and linked with the product's other
+    objects (the body-slot build included) into lib/variants/<name>/."""
     variant = _variant()
     if variant:
         prev = os.environ.pop("TRL_VARIANT")
@@ -86,6 +88,7 @@ def build_library(force=False, verbose=False):
     csrc = os.path.join(_PKG, "csrc")
     units = [("trl_step.cu", []), ("trl_step_cg.cu", ["-Xptxas", "-dlcm=cg"]), ("trl_step_ts.cu", []), ("trl_step_ts_cg.cu", ["-Xptxas", "-dlcm=cg"]),
              ("trl_step_ps.cu", []), ("trl_step_ps_cg.cu", ["-Xptxas", "-dlcm=cg"]),
+             ("trl_step_bs.cu", []), ("trl_step_bs_cg.cu", ["-Xptxas", "-dlcm=cg"]),
              ("trl_host.cu", []), ("trl_train.cu", []), ("trl_checkpoint.cu", []),
              ("trl_comm.cu", []), ("trl_probe.cu", []), ("trl_tc_policy.cu", []), ("ref_loader.cpp", [])]
     deps = [os.path.join(csrc, f) for f in os.listdir(csrc)]
@@ -138,6 +141,7 @@ EXPORTS = [
     "trl_checkpoint_save", "trl_create_from_checkpoint", "trl_trainer_params", "trl_env_policy",
     "trl_load_physics", "trl_set_env_physics", "trl_env_physics", "trl_eval_stats_phys",
     "trl_set_env_eval", "trl_env_eval", "trl_eval_stats_mode",
+    "trl_load_body", "trl_set_env_body", "trl_env_body", "trl_eval_stats_body",
 ]
 
 
@@ -312,6 +316,27 @@ class BatchedScenario:
         self._ck(self.L.trl_env_physics(self.h, _p(cur), _p(nxt), self.num_envs))
         return cur, nxt
 
+    def LoadBody(self, slot, path):
+        """a character file of the reference's format (as -character_file) into body slot 1..7; envs move to it with SetEnvBody.  The
+        file must have the scene's topology and controllers; its masses, dimensions, joint limits and PD gains may differ.  A relative
+        path (and the controller files it names) refers to the scenario's data_root."""
+        self._ck(self.L.trl_load_body(self.h, int(slot), os.fspath(path).encode()))
+
+    def SetEnvBody(self, slots, env_ids=None):
+        """env_ids[k] (default: env k) runs on body slot slots[k] from its next episode reset on"""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        ids = None if env_ids is None else np.ascontiguousarray(env_ids, dtype=np.int32).ravel()
+        if ids is not None and ids.size != s.size:
+            raise ValueError("SetEnvBody: one slot per env id")
+        self._ck(self.L.trl_set_env_body(self.h, _p(ids), _p(s), int(s.size)))
+
+    def EnvBody(self):
+        """(current, assigned): per env, the body slot of its present episode and the one it gets at its next reset"""
+        cur = np.zeros(self.num_envs, np.int32)
+        nxt = np.zeros(self.num_envs, np.int32)
+        self._ck(self.L.trl_env_body(self.h, _p(cur), _p(nxt), self.num_envs))
+        return cur, nxt
+
     def SetEnvEval(self, flags, env_ids=None):
         """env_ids[k] (default: env k) of an exploration scenario evaluates its policy slot's current net, exploration off and no
         tuples recorded, from its next episode reset on if flags[k] is true; it explores again from its next reset if false"""
@@ -478,12 +503,16 @@ class BatchedScenario:
     def GetNumEnvSteps(self):
         return self._stats()["steps"]
 
-    def GetEvalStats(self, slot=0, terrain=None, physics=None, mode=None):
+    def GetEvalStats(self, slot=0, terrain=None, physics=None, mode=None, body=None):
         """cycles / episodes / avg_dist / env-steps of the envs now on policy slot `slot` (None: any) whose present ground comes from
-        terrain slot `terrain` (None: any), whose present episode runs on physics slot `physics` (None: any) and in mode `mode`
-        (TRL_MODE_POLI_EVAL = 0 evaluates, TRL_MODE_EXPLORE = 1 explores; None: any)"""
+        terrain slot `terrain` (None: any), whose present episode runs on physics slot `physics` (None: any), in mode `mode`
+        (TRL_MODE_POLI_EVAL = 0 evaluates, TRL_MODE_EXPLORE = 1 explores; None: any) and on body slot `body` (None: any)"""
         c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
-        if mode is not None:
+        if body is not None:
+            rc = self.L.trl_eval_stats_body(self.h, -1 if mode is None else int(mode), -1 if slot is None else int(slot),
+                                            -1 if terrain is None else int(terrain), -1 if physics is None else int(physics), int(body),
+                                            C.byref(c), C.byref(e), C.byref(a), C.byref(s))
+        elif mode is not None:
             rc = self.L.trl_eval_stats_mode(self.h, int(mode), -1 if slot is None else int(slot), -1 if terrain is None else int(terrain),
                                             -1 if physics is None else int(physics), C.byref(c), C.byref(e), C.byref(a), C.byref(s))
         elif physics is not None:
@@ -497,10 +526,10 @@ class BatchedScenario:
         self._ck(rc)
         return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
 
-    def GetDistLog(self, slot=None, terrain=None, physics=None, mode=None):
-        """(distances, env ids) of the episodes logged so far; slot / terrain / physics / mode: only the entries of envs now on that
-        policy slot / whose present ground comes from that terrain slot / whose present episode runs on that physics slot / whose
-        present episode runs in that mode (0 evaluates, 1 explores).  Every filter reads the env's present assignment, not the one of
+    def GetDistLog(self, slot=None, terrain=None, physics=None, mode=None, body=None):
+        """(distances, env ids) of the episodes logged so far; slot / terrain / physics / mode / body: only the entries of envs now on
+        that policy slot / whose present ground comes from that terrain slot / whose present episode runs on that physics slot / whose
+        present episode runs in that mode (0 evaluates, 1 explores) / whose present episode runs on that body slot.  Every filter reads the env's present assignment, not the one of
         the logged episode: only evaluating episodes log a distance, but an env that has gone back to exploring keeps its entries,
         which mode=1 then returns and mode=0 drops."""
         d = C.c_void_p(); e = C.c_void_p(); n = C.c_int(0)
@@ -520,6 +549,9 @@ class BatchedScenario:
             dist, env = dist[keep], env[keep]
         if mode is not None:
             keep = self.EnvEval()[0][env] == (int(mode) == 0)
+            dist, env = dist[keep], env[keep]
+        if body is not None:
+            keep = self.EnvBody()[0][env] == body
             dist, env = dist[keep], env[keep]
         return dist, env
 

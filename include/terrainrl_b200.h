@@ -247,6 +247,32 @@ int trl_set_env_eval(trl_handle* h, const int32_t* env_ids, const int32_t* flags
 int trl_env_eval(trl_handle* h, int32_t* current, int32_t* assigned, int n);
 int trl_eval_stats_mode(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int64_t* cycles, int64_t* episodes,
                         double* avg_dist, int64_t* env_steps);
+/* Body slots (any mode; with or without trainers, policy, terrain or physics slots, or evaluation envs): up to 8 bodies of the scene's
+ * character per handle.  Slot 0 is the scene's own body; slots 1..7 start empty.  With the same seeds, env i on body slot b computes
+ * bit for bit what env i computes in a handle created from the same arguments plus -character_file=<slot b's file>.
+ *   trl_load_body        a character file of the reference's format into slot 1..7: per link its Skeleton AttachX/Y and LimLow/LimHigh,
+ *                        BodyDefs Mass, AttachX/Y, Theta, Param0/1, PDControllers Kp, Kd, TorqueLim, TargetTheta, TargetVel and
+ *                        UseWorldCoord.  A relative path (and the controller files the file names) refers to trl_create's data_root;
+ *                        a handle made by trl_create_from_pack or trl_create_from_checkpoint has none, and resolves relative paths
+ *                        against the process's working directory (give absolute paths there).
+ *                        Refused, handle unchanged, for slot 0 or >= 8, a null path, malformed JSON, a joint count, joint Type or
+ *                        Parent, or body Shape other than the scene's, a Controllers section whose files resolve to other parameter
+ *                        sets or whose Actions, DefaultAction or gravity-compensation / virtual-force flags differ, a non-finite number,
+ *                        Mass <= 0, a box size <= 0, Kp, Kd or TorqueLim < 0, a body that reaches more than 1.75 m from its root joint
+ *                        (UpdateGround keeps the ground from 2 m behind the root on, and the broad phase reads 0.25 m beyond the
+ *                        reach), or a slot that is some env's present or assigned body.
+ *   trl_set_env_body     env_ids[k] (NULL: env k) -> slots[k] for k < n; every env starts on slot 0.  Refused, with nothing changed, for
+ *                        an env id or slot out of range, n > num_envs or an empty slot.  Takes effect at the env's next episode reset
+ *                        (a fall inside trl_update, trl_reset, trl_seed_terrain): an episode never mixes two bodies.
+ *   trl_env_body         per env (first n), the slot of its present episode and the slot it gets at its next reset.
+ *   trl_eval_stats_body  trl_eval_stats_mode(mode, policy_slot, terrain_slot, phys_slot) over the envs whose present episode runs on
+ *                        body slot body_slot (-1 = any: then it is trl_eval_stats_mode's).  The other statistics entries keep counting
+ *                        every env. */
+int trl_load_body(trl_handle* h, int slot, const char* character_json_path);
+int trl_set_env_body(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n);
+int trl_env_body(trl_handle* h, int32_t* current, int32_t* assigned, int n);
+int trl_eval_stats_body(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int body_slot, int64_t* cycles,
+                        int64_t* episodes, double* avg_dist, int64_t* env_steps);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
