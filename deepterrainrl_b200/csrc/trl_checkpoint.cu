@@ -198,6 +198,11 @@ int handle_state(trl_handle* h, std::vector<CkptSection>* out) {
         host("env_body_host", 1, h->env_body_host.data(), n * 4);
         fixed("env_body", 1, h->env_body, 2 * n * 4);
     }
+    if (h->ranges.env_draws) {     // ranged slots: likewise written only once one is loaded
+        fixed("env_bdraw", 0, h->ranges.env_bdraw, n * sizeof(BodyConst));
+        fixed("env_pdraw", 0, h->ranges.env_pdraw, n * sizeof(PhysParams));
+        fixed("env_draws", 0, h->ranges.env_draws, 2 * n * 8);
+    }
     fixed("B.d", 3, B.d, (size_t)D_NUM_FIELDS * n * 8);
     fixed("B.i", 1, B.i, (size_t)I_NUM_PLANES * n * 4);
     fixed("B.terrain", 2, B.terrain, n * 2 * kTerrainCap * 4);
@@ -308,6 +313,12 @@ int save_impl(trl_handle* h, const char* path, const void* user, size_t user_byt
             if (h->body_loaded[s]) mask |= 1 << s;
         build.push_back(blob_of("body_loaded", 1, &mask, 1));
         build.push_back(blob_of("body_table", 0, h->body, kMaxBodySlots));
+    }
+    if (h->ranges.env_draws) {     // the ranged slots' hi tables (their lo tables are the slot tables above)
+        const int32_t masks[2] = {(int32_t)h->ranges.body_ranged, (int32_t)h->ranges.phys_ranged};
+        build.push_back(blob_of("ranges", 1, masks, 2));
+        build.push_back(blob_of("range_body_hi", 0, h->ranges.body_hi, kMaxBodySlots));
+        build.push_back(blob_of("range_phys_hi", 0, h->ranges.phys_hi, kMaxPhysSlots));
     }
     build.insert(build.begin() + 1, blob_of("meta", 0, &m, 1));
     build.push_back(blob_of("user", 0, (const unsigned char*)user, user_bytes));
@@ -458,11 +469,36 @@ trl_handle* load_impl(const char* path, int device, trl_trainer** trainers_out, 
         const auto* tb = need("body_table", sizeof(BodyConst) * kMaxBodySlots);
         int32_t mask = 0;
         if (lb->size() == 4) std::memcpy(&mask, lb->data(), 4);
-        if (!tb || lb->size() != 4 || mask == 0 || (mask & ~0xfe)) return bail("body slots: table or slot mask missing or malformed");
+        // a handle whose only ranged slots are physics slots runs the body-slot build without a body slot
+        if (!tb || lb->size() != 4 || (mask == 0 && !need("ranges", 0)) || (mask & ~0xfe))
+            return bail("body slots: table or slot mask missing or malformed");
         std::vector<BodyConst> table(kMaxBodySlots);
         std::memcpy(table.data(), tb->data(), sizeof(BodyConst) * kMaxBodySlots);
         for (int s = 1; s < kMaxBodySlots; ++s)
             if ((mask & (1 << s)) && trl_set_body_slot(h, s, table[s])) return bail("");
+    }
+    if (const auto* rb = need("ranges", 0)) {         // the ranged slots: their lo tables are the slots restored above
+        const auto* bh = need("range_body_hi", sizeof(BodyConst) * kMaxBodySlots);
+        const auto* ph = need("range_phys_hi", sizeof(PhysParams) * kMaxPhysSlots);
+        int32_t masks[2] = {0, 0};
+        if (rb->size() == 8) std::memcpy(masks, rb->data(), 8);
+        if (!bh || !ph || rb->size() != 8 || (masks[0] & ~0xfe) || (masks[1] & ~0xfe) || !need("body_loaded", 0))
+            return bail("ranged slots: tables or slot masks missing or malformed");
+        std::vector<BodyConst> body_hi(kMaxBodySlots);
+        std::vector<PhysParams> phys_hi(kMaxPhysSlots);
+        std::memcpy(body_hi.data(), bh->data(), bh->size());
+        std::memcpy(phys_hi.data(), ph->data(), ph->size());
+        if (trl_enable_ranges(h)) return bail("");
+        for (int s = 1; s < kMaxBodySlots; ++s) {
+            if (!(masks[0] & (1 << s))) continue;
+            if (!h->body_loaded[s]) return bail("ranged body slot " + std::to_string(s) + " has no lo table");
+            if (trl_set_body_range(h, s, h->body[s], body_hi[s])) return bail("");
+        }
+        for (int s = 1; s < kMaxPhysSlots; ++s) {
+            if (!(masks[1] & (1 << s))) continue;
+            if (!h->phys_loaded[s]) return bail("ranged physics slot " + std::to_string(s) + " has no lo table");
+            if (trl_set_phys_range(h, s, h->phys[s], phys_hi[s])) return bail("");
+        }
     }
     if ((m.policies || m.trainers || eb) && !h->mc.has_net) return bail("the scene has no policy net");
     if (eb && trl_enable_env_eval(h)) return bail("");

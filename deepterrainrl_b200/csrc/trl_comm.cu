@@ -272,6 +272,7 @@ int trl_comm_init(trl_handle* h, const void* id128, int rank, int world) {
     if (!h) return trl_fail("trl_comm_init: null handle");
     if (h->comm) return trl_fail("trl_comm_init: the handle already has a communicator");
     if (h->env_eval) return trl_fail("trl_comm_init: the handle has evaluation envs (trl_set_env_eval)");
+    if (h->ranges.body_ranged || h->ranges.phys_ranged) return trl_fail("trl_comm_init: the handle has ranged slots (trl_load_body_range / trl_load_physics_range)");
     if (!id128 || world < 1 || rank < 0 || rank >= world) return trl_fail("trl_comm_init: bad rank / world / id");
     if (load_nccl()) return 1;
     CCK(cudaSetDevice(h->device));
@@ -289,6 +290,7 @@ int trl_comm_init_external(trl_handle* h, const trl_collectives* coll, int rank,
     if (!h) return trl_fail("trl_comm_init_external: null handle");
     if (h->comm) return trl_fail("trl_comm_init_external: the handle already has a communicator");
     if (h->env_eval) return trl_fail("trl_comm_init_external: the handle has evaluation envs (trl_set_env_eval)");
+    if (h->ranges.body_ranged || h->ranges.phys_ranged) return trl_fail("trl_comm_init_external: the handle has ranged slots (trl_load_body_range / trl_load_physics_range)");
     if (!coll || !coll->all_gather || !coll->broadcast || !coll->all_reduce_sum_f64 || world < 1 || rank < 0 || rank >= world)
         return trl_fail("trl_comm_init_external: bad rank / world / callbacks");
     auto* c = new trl_comm();

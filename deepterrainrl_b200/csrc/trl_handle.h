@@ -91,6 +91,10 @@ struct trl_handle {
     bool body_loaded[trl::kMaxBodySlots] = {};                 // [0] unused
     std::vector<int> env_body_host;                            // the assignment of every env (row 1 of env_body)
     int* env_body = nullptr;                                   // device [2][n]: slot of the present episode, slot from the next reset on
+    // ranged slots (trl_load_body_range, trl_load_physics_range): body[s] / phys[s] hold a ranged slot's lo numbers, ranges its hi
+    // numbers, its bit in ranges.body_ranged / phys_ranged, and the per-env draw tables (allocated at the first ranged slot, with
+    // the body-slot build; null before)
+    trl::RangeTables ranges = {};
     std::string data_root;                                     // trl_create's: the directory relative character and controller paths refer to
     int64_t launches = 0;
     std::map<long long, cudaGraphExec_t> graphs;   // keyed by the bit pattern of dt
@@ -138,6 +142,11 @@ int trl_set_terrain_slot(trl_handle* h, int slot, int type, std::vector<double> 
 extern "C" int trl_enable_env_eval(trl_handle* h);
 // body slot `slot` >= 1 holds `b` (trl_load_body once the file is read and checked), and the handle moves onto the body-slot build
 extern "C" int trl_set_body_slot(trl_handle* h, int slot, const trl::BodyConst& b);
+// ranged slots: the per-env draw tables and the body-slot build (trl_load_body_range / trl_load_physics_range, a checkpoint's restore);
+// body / physics slot `slot` >= 1 drawn in [lo, hi] at every episode reset, after the loaders' checks of the two ends
+extern "C" int trl_enable_ranges(trl_handle* h);
+extern "C" int trl_set_body_range(trl_handle* h, int slot, const trl::BodyConst& lo, const trl::BodyConst& hi);
+extern "C" int trl_set_phys_range(trl_handle* h, int slot, const trl::PhysParams& lo, const trl::PhysParams& hi);
 
 // One array of a checkpoint (trl_checkpoint.cu): `bytes` of device memory at `dev`, or of host memory at `host` when dev is null.
 // `cap` is the room there is: a restore accepts up to cap bytes (the replay rows, the tuple block and the distance log are saved up

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
+#include <cstddef>
+#include <type_traits>
 #include <cstdio>
 #include <cstring>
 #include <map>
@@ -51,10 +53,12 @@ void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStre
 namespace trl {
 cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t upload_body(const BodyConst* body, int* env_body);
+cudaError_t upload_ranges(const RangeTables& r);
 }
 namespace trl_cg {
 cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
+cudaError_t upload_ranges(const trl::RangeTables& r);
 }
 namespace trl_ts = trl;
 namespace trl_ts_cg = trl_cg;
@@ -93,6 +97,7 @@ namespace trl_bs {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
 cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
+cudaError_t upload_ranges(const trl::RangeTables& r);
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 void launch_reset(const trl::Buffers& B, const uint64_t* seeds, const int* env_ids, int count, int reseed, cudaStream_t st);
@@ -102,6 +107,7 @@ namespace trl_bs_cg {
 cudaError_t upload_model(const trl::ModelConst& mc, const trl::TerrainSlot* terrain);
 cudaError_t upload_phys(const trl::PhysParams* phys, int* env_phys, int* env_eval);
 cudaError_t upload_body(const trl::BodyConst* body, int* env_body);
+cudaError_t upload_ranges(const trl::RangeTables& r);
 cudaError_t configure_step_kernels();
 void launch_step(const trl::Buffers& B, double h, int flags, int lists, cudaStream_t st, int group = 0, int n_groups = 1);
 }  // namespace trl_bs_cg
@@ -115,7 +121,7 @@ struct trl_handle;
 static const trl_handle* g_model_owner = nullptr;    // whose ModelConst currently sits in the __constant__ copies
 static int g_device = -1;                             // the one device this process drives (set by the first handle)
 static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* terrain, const PhysParams* phys, int* env_phys, int* env_eval,
-                                    const BodyConst* body, int* env_body) {
+                                    const BodyConst* body, int* env_body, const RangeTables& ranges) {
     cudaError_t e = trl::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_cg::upload_model(mc, terrain);
     if (e == cudaSuccess) e = trl_ts::upload_model(mc, terrain);
@@ -131,7 +137,9 @@ static cudaError_t upload_model_all(const ModelConst& mc, const TerrainSlot* ter
     if (e == cudaSuccess) e = trl_bs_cg::upload_phys(phys, env_phys, env_eval);
 #endif
     if (e == cudaSuccess) e = trl_bs::upload_body(body, env_body);
-    return e != cudaSuccess ? e : trl_bs_cg::upload_body(body, env_body);
+    if (e == cudaSuccess) e = trl_bs_cg::upload_body(body, env_body);
+    if (e == cudaSuccess) e = trl_bs::upload_ranges(ranges);
+    return e != cudaSuccess ? e : trl_bs_cg::upload_ranges(ranges);
 }
 
 // the per-link numbers of the scene's body (slot 0 of the body table), as fill_model derived them from the character file
@@ -181,7 +189,7 @@ static int ensure_model_only(trl_handle* h) {
     std::memcpy(h->terrain[0].params, h->mc.terrain_params, sizeof(h->mc.terrain_params));
     h->phys[0] = h->mc.phys;                      // and slot 0 of the physics table its own physics
     h->body[0] = body_of(h->mc);                  // and slot 0 of the body table its own body
-    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys, h->env_eval, h->body, h->env_body) != cudaSuccess) return 1;
+    if (upload_model_all(h->mc, h->terrain, h->phys, h->env_phys, h->env_eval, h->body, h->env_body, h->ranges) != cudaSuccess) return 1;
     g_model_owner = h;
     return 0;
 }
@@ -1537,20 +1545,9 @@ int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episo
 
 static bool phys_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxPhysSlots && h->phys_loaded[slot]); }
 
-int trl_load_physics(trl_handle* h, int slot, const double* p, int vertex_contacts) {
-    const std::string who = "trl_load_physics";
-    if (!h) return fail(who + ": null handle");
-    if (slot < 1 || slot >= kMaxPhysSlots)
-        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxPhysSlots - 1) + "; slot 0 is the scene's physics, set by trl_set_phys_params)");
-    if (!p) return fail(who + ": null parameter array");
-    static const char* names[7] = {"kn", "dn", "mu", "v_eps", "contact_tol", "k_lim", "d_lim"};
-    for (int k = 0; k < 7; ++k)
-        if (!std::isfinite(p[k])) return fail(who + ": " + names[k] + " is not finite");
-    for (int k : {0, 1, 2, 5, 6})
-        if (p[k] < 0.0) return fail(who + ": " + names[k] + " = " + std::to_string(p[k]) + " is negative");
-    if (!(p[3] > 0.0)) return fail(who + ": v_eps = " + std::to_string(p[3]) + " must be positive");
-    if (p[4] * std::sqrt(1.0 + kMaxSlope * kMaxSlope) > kClearMargin)
-        return fail(who + ": contact_tol = " + std::to_string(p[4]) + " exceeds what the broad phase covers (contact_tol * sqrt(1 + 25^2) <= 0.05)");
+// physics slot `slot` >= 1 holds `q` (its numbers checked), fixed or (hi non-null) ranged up to *hi, and the handle moves onto the
+// physics-slot build
+static int set_phys_slot(trl_handle* h, const std::string& who, int slot, const PhysParams& q, const PhysParams* hi = nullptr) {
     if (drain(h)) return 1;
     if (!h->env_phys) {     // first slot: from now on the step launches run the physics-slot build
         int* d = nullptr;
@@ -1559,10 +1556,41 @@ int trl_load_physics(trl_handle* h, int slot, const double* p, int vertex_contac
         h->env_phys_host.assign((size_t)h->n, 0);
         destroy_graphs(h);
     }
-    h->phys[slot] = PhysParams{p[0], p[1], p[2], p[3], p[4], p[5], p[6], vertex_contacts ? 1 : 0};
+    h->phys[slot] = q;
     h->phys_loaded[slot] = true;
+    if (hi) {
+        h->ranges.phys_hi[slot] = *hi;
+        h->ranges.phys_ranged |= 1u << slot;
+    } else {
+        h->ranges.phys_ranged &= ~(1u << slot);
+    }
     g_model_owner = nullptr;
     return ensure_model(h) ? fail(who + ": physics table upload failed") : 0;
+}
+
+static const char* kPhysNames[7] = {"kn", "dn", "mu", "v_eps", "contact_tol", "k_lim", "d_lim"};
+
+// the checks trl_load_physics makes of a slot's seven constants (`what`: "" or the name of a range's end, for the messages)
+static int check_p7(const std::string& who, const double* p, const std::string& what) {
+    const char* const* names = kPhysNames;
+    for (int k = 0; k < 7; ++k)
+        if (!std::isfinite(p[k])) return fail(who + ": " + what + names[k] + " is not finite");
+    for (int k : {0, 1, 2, 5, 6})
+        if (p[k] < 0.0) return fail(who + ": " + what + names[k] + " = " + std::to_string(p[k]) + " is negative");
+    if (!(p[3] > 0.0)) return fail(who + ": " + what + "v_eps = " + std::to_string(p[3]) + " must be positive");
+    if (p[4] * std::sqrt(1.0 + kMaxSlope * kMaxSlope) > kClearMargin)
+        return fail(who + ": " + what + "contact_tol = " + std::to_string(p[4]) + " exceeds what the broad phase covers (contact_tol * sqrt(1 + 25^2) <= 0.05)");
+    return 0;
+}
+
+int trl_load_physics(trl_handle* h, int slot, const double* p, int vertex_contacts) {
+    const std::string who = "trl_load_physics";
+    if (!h) return fail(who + ": null handle");
+    if (slot < 1 || slot >= kMaxPhysSlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxPhysSlots - 1) + "; slot 0 is the scene's physics, set by trl_set_phys_params)");
+    if (!p) return fail(who + ": null parameter array");
+    if (check_p7(who, p, "")) return 1;
+    return set_phys_slot(h, who, slot, PhysParams{p[0], p[1], p[2], p[3], p[4], p[5], p[6], vertex_contacts ? 1 : 0});
 }
 
 int trl_set_env_physics(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
@@ -1739,29 +1767,32 @@ static bool body_ok(const BodyConst& b, int nj, std::string* why) {
     return true;
 }
 
+// the per-env body slots, every env on slot 0: from now on the step launches run the body-slot build (drained by the caller)
+static int enable_body_slots(trl_handle* h) {
+    if (h->env_body) return 0;
+    int* d = nullptr;
+    CK(dalloc(h, &d, 2 * (size_t)h->n));
+    h->env_body = d;
+    h->env_body_host.assign((size_t)h->n, 0);
+    destroy_graphs(h);
+    return 0;
+}
+
 int trl_set_body_slot(trl_handle* h, int slot, const BodyConst& b) {
     std::string why;
     if (slot < 1 || slot >= kMaxBodySlots) return fail("body slot " + std::to_string(slot) + " out of range");
     if (!body_ok(b, h->mc.nj, &why)) return fail("body slot " + std::to_string(slot) + ": " + why);
     if (drain(h)) return 1;
-    if (!h->env_body) {     // first slot: from now on the step launches run the body-slot build
-        int* d = nullptr;
-        CK(dalloc(h, &d, 2 * (size_t)h->n));
-        h->env_body = d;
-        h->env_body_host.assign((size_t)h->n, 0);
-        destroy_graphs(h);
-    }
+    if (enable_body_slots(h)) return 1;
     h->body[slot] = b;
     h->body_loaded[slot] = true;
+    h->ranges.body_ranged &= ~(1u << slot);
     g_model_owner = nullptr;
     return ensure_model(h) ? fail("trl_load_body: body table upload failed") : 0;
 }
 
-int trl_load_body(trl_handle* h, int slot, const char* character_json_path) {
-    const std::string who = "trl_load_body";
-    if (!h) return fail(who + ": null handle");
-    if (slot < 1 || slot >= kMaxBodySlots)
-        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxBodySlots - 1) + "; slot 0 is the scene's body)");
+// the body a character file describes, checked as trl_load_body checks it (topology, controllers, numbers, reach)
+static int read_body(trl_handle* h, const std::string& who, const char* character_json_path, BodyConst* out) {
     if (!character_json_path) return fail(who + ": null path");
     const ModelConst& sm = h->mc;
     // the scene with this file's character records: fill_model derives from it what it derives for a handle created with
@@ -1816,15 +1847,31 @@ int trl_load_body(trl_handle* h, int slot, const char* character_json_path) {
     if (bm.reach > kMaxReach)
         return fail(who + ": the body reaches " + std::to_string(bm.reach) + " m from its root joint, more than the " + std::to_string(kMaxReach) +
                     " m the ground window covers (UpdateGround keeps 2 m behind the root; the broad phase reads reach + 0.25 m)");
+    *out = body_of(bm);
+    return 0;
+}
+
+// refused while `slot` is some env's present or assigned slot (`cur_dev`: the device [2][n] array, null when there is none)
+static int slot_unused(trl_handle* h, const std::string& who, int slot, const int* cur_dev, const std::vector<int>& assigned, const char* what) {
+    if (!cur_dev) return 0;
     if (drain(h)) return 1;
-    if (h->env_body) {
-        std::vector<int> cur((size_t)h->n);
-        CK(cudaMemcpy(cur.data(), h->env_body, cur.size() * 4, cudaMemcpyDeviceToHost));
-        for (int e = 0; e < h->n; ++e)
-            if (cur[e] == slot || h->env_body_host[e] == slot)
-                return fail(who + ": slot " + std::to_string(slot) + " is in use (env " + std::to_string(e) + "'s present or assigned body)");
-    }
-    return trl_set_body_slot(h, slot, body_of(bm));
+    std::vector<int> cur((size_t)h->n);
+    CK(cudaMemcpy(cur.data(), cur_dev, cur.size() * 4, cudaMemcpyDeviceToHost));
+    for (int e = 0; e < h->n; ++e)
+        if (cur[e] == slot || assigned[e] == slot)
+            return fail(who + ": slot " + std::to_string(slot) + " is in use (env " + std::to_string(e) + "'s present or assigned " + what + ")");
+    return 0;
+}
+
+int trl_load_body(trl_handle* h, int slot, const char* character_json_path) {
+    const std::string who = "trl_load_body";
+    if (!h) return fail(who + ": null handle");
+    if (slot < 1 || slot >= kMaxBodySlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxBodySlots - 1) + "; slot 0 is the scene's body)");
+    BodyConst b;
+    if (read_body(h, who, character_json_path, &b)) return 1;
+    if (slot_unused(h, who, slot, h->env_body, h->env_body_host, "body")) return 1;
+    return trl_set_body_slot(h, slot, b);
 }
 
 int trl_set_env_body(trl_handle* h, const int32_t* env_ids, const int32_t* slots, int n) {
@@ -1874,6 +1921,165 @@ int trl_eval_stats_body(trl_handle* h, int mode, int policy_slot, int terrain_sl
     const bool filter = body_slot >= 0 && h->env_body;
     return eval_stats_mode(h, who, mode, policy_slot, terrain_slot, phys_slot, cycles, episodes, avg_dist, env_steps, filter ? h->env_body : nullptr,
                            filter ? body_slot : -1);
+}
+
+// ---- ranged slots (trl_types.h: kBodyDrawTag)
+// the per-env draw tables, at the handle's first ranged slot; a ranged slot is drawn where the body-slot build restages bodies, so the
+// handle moves onto that build (drained by the caller)
+int trl_enable_ranges(trl_handle* h) {
+    if (h->ranges.env_draws) return 0;
+    if (enable_body_slots(h)) return 1;
+    const size_t n = (size_t)h->n;
+    CK(dalloc(h, &h->ranges.env_bdraw, n));
+    CK(dalloc(h, &h->ranges.env_pdraw, n));
+    CK(dalloc(h, &h->ranges.env_draws, 2 * n));
+    return 0;
+}
+
+// what a ranged body slot's two ends must satisfy: each a body trl_set_body_slot accepts, the same numbers but for the four drawn
+// fields (and what fill_model derives from them), lo <= hi in those
+static int check_body_range(const std::string& who, const BodyConst& lo, const BodyConst& hi, int nj) {
+    std::string why;
+    if (!body_ok(lo, nj, &why)) return fail(who + ": lo: " + why);
+    if (!body_ok(hi, nj, &why)) return fail(who + ": hi: " + why);
+    struct F { const char* name; size_t off; int per_link; bool is_int; };
+#define TRL_F(f, name, k) F{name, offsetof(BodyConst, f), k, std::is_same<decltype(+lo.f[0]), int>::value}
+    static const F fixed[] = {TRL_F(attach_x, "Skeleton AttachX", 1), TRL_F(attach_y, "Skeleton AttachY", 1), TRL_F(lim_lo, "LimLow", 1),
+                              TRL_F(lim_hi, "LimHigh", 1), TRL_F(has_limit, "joint limit", 1), TRL_F(body_ax, "BodyDefs AttachX", 1),
+                              TRL_F(body_ay, "BodyDefs AttachY", 1), TRL_F(body_theta, "Theta", 1), TRL_F(body_cos, "Theta", 1),
+                              TRL_F(body_sin, "Theta", 1), TRL_F(half_x, "Param0 (box size)", 1), TRL_F(half_y, "Param1 (box size)", 1),
+                              TRL_F(corner_lx, "box corner", 4), TRL_F(corner_ly, "box corner", 4), TRL_F(target_theta0, "TargetTheta", 1),
+                              TRL_F(target_vel, "TargetVel", 1), TRL_F(world_pd, "UseWorldCoord", 1)};
+#undef TRL_F
+    for (const F& f : fixed) {
+        const size_t w = f.is_int ? 4 : 8;
+        const unsigned char* a = reinterpret_cast<const unsigned char*>(&lo) + f.off;
+        const unsigned char* b = reinterpret_cast<const unsigned char*>(&hi) + f.off;
+        for (int i = 0; i < f.per_link * nj; ++i)
+            if (std::memcmp(a + i * w, b + i * w, w) != 0)
+                return fail(who + ": the lo and hi bodies differ in " + f.name + " of link " + std::to_string(i / f.per_link) +
+                            " (only Mass, Kp, Kd and TorqueLim are drawn)");
+    }
+    if (std::memcmp(&lo.reach, &hi.reach, sizeof(lo.reach)) != 0) return fail(who + ": the lo and hi bodies differ in their reach");
+    const double* l[kBodyDrawFields] = {lo.mass, lo.kp, lo.kd, lo.torque_lim};
+    const double* u[kBodyDrawFields] = {hi.mass, hi.kp, hi.kd, hi.torque_lim};
+    static const char* names[kBodyDrawFields] = {"Mass", "Kp", "Kd", "TorqueLim"};
+    for (int f = 0; f < kBodyDrawFields; ++f)
+        for (int j = 0; j < nj; ++j)
+            if (!(l[f][j] <= u[f][j]))
+                return fail(who + ": " + names[f] + " of link " + std::to_string(j) + ": lo " + std::to_string(l[f][j]) + " > hi " + std::to_string(u[f][j]));
+    return 0;
+}
+
+int trl_set_body_range(trl_handle* h, int slot, const BodyConst& lo, const BodyConst& hi) {
+    const std::string who = "trl_load_body_range";
+    if (slot < 1 || slot >= kMaxBodySlots) return fail(who + ": slot " + std::to_string(slot) + " out of range");
+    if (check_body_range(who, lo, hi, h->mc.nj)) return 1;
+    if (drain(h)) return 1;
+    if (trl_enable_ranges(h)) return 1;
+    h->body[slot] = lo;
+    h->body_loaded[slot] = true;
+    h->ranges.body_hi[slot] = hi;
+    h->ranges.body_ranged |= 1u << slot;
+    g_model_owner = nullptr;
+    return ensure_model(h) ? fail("trl_load_body_range: body table upload failed") : 0;
+}
+
+int trl_load_body_range(trl_handle* h, int slot, const char* lo_path, const char* hi_path) {
+    const std::string who = "trl_load_body_range";
+    if (!h) return fail(who + ": null handle");
+    if (h->comm) return fail(who + ": ranged slots do not run with a communicator");
+    if (slot < 1 || slot >= kMaxBodySlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxBodySlots - 1) + "; slot 0 is the scene's body)");
+    BodyConst lo, hi;
+    if (read_body(h, who + ": lo", lo_path, &lo) || read_body(h, who + ": hi", hi_path, &hi)) return 1;
+    if (slot_unused(h, who, slot, h->env_body, h->env_body_host, "body")) return 1;
+    return trl_set_body_range(h, slot, lo, hi);
+}
+
+int trl_set_phys_range(trl_handle* h, int slot, const PhysParams& lo, const PhysParams& hi) {
+    const std::string who = "trl_load_physics_range";
+    if (slot < 1 || slot >= kMaxPhysSlots) return fail(who + ": slot " + std::to_string(slot) + " out of range");
+    const double l[7] = {lo.kn, lo.dn, lo.mu, lo.v_eps, lo.contact_tol, lo.k_lim, lo.d_lim};
+    const double u[7] = {hi.kn, hi.dn, hi.mu, hi.v_eps, hi.contact_tol, hi.k_lim, hi.d_lim};
+    if (check_p7(who, l, "lo ") || check_p7(who, u, "hi ")) return 1;
+    for (int k = 0; k < 7; ++k)
+        if (!(l[k] <= u[k])) return fail(who + ": " + kPhysNames[k] + ": lo " + std::to_string(l[k]) + " > hi " + std::to_string(u[k]));
+    if (lo.vertex_contacts != hi.vertex_contacts || (lo.vertex_contacts & ~1)) return fail(who + ": vertex_contacts malformed");
+    if (drain(h)) return 1;
+    if (trl_enable_ranges(h)) return 1;
+    return set_phys_slot(h, who, slot, lo, &hi);
+}
+
+int trl_load_physics_range(trl_handle* h, int slot, const double* lo7, const double* hi7, int vertex_contacts) {
+    const std::string who = "trl_load_physics_range";
+    if (!h) return fail(who + ": null handle");
+    if (h->comm) return fail(who + ": ranged slots do not run with a communicator");
+    if (slot < 1 || slot >= kMaxPhysSlots)
+        return fail(who + ": slot " + std::to_string(slot) + " out of range (1.." + std::to_string(kMaxPhysSlots - 1) + "; slot 0 is the scene's physics, set by trl_set_phys_params)");
+    if (!lo7 || !hi7) return fail(who + ": null parameter array");
+    if (slot_unused(h, who, slot, h->env_phys, h->env_phys_host, "physics")) return 1;
+    const int vc = vertex_contacts ? 1 : 0;
+    return trl_set_phys_range(h, slot, PhysParams{lo7[0], lo7[1], lo7[2], lo7[3], lo7[4], lo7[5], lo7[6], vc},
+                              PhysParams{hi7[0], hi7[1], hi7[2], hi7[3], hi7[4], hi7[5], hi7[6], vc});
+}
+
+// every env's present slot (row 0 of a device [2][n] array; null: every env on slot 0) and draw count of one kind (0 body, 1 physics)
+static int present_slots(trl_handle* h, const int* dev, int kind, std::vector<int>* cur, std::vector<long long>* draws) {
+    const size_t n = (size_t)h->n;
+    cur->assign(n, 0);
+    draws->assign(n, 0);
+    if (drain(h)) return 1;
+    if (dev) CK(cudaMemcpy(cur->data(), dev, n * 4, cudaMemcpyDeviceToHost));
+    if (h->ranges.env_draws) CK(cudaMemcpy(draws->data(), h->ranges.env_draws + kind * n, n * 8, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int trl_env_body_draws(trl_handle* h, double* out, int64_t* draws) {
+    if (!h) return fail("trl_env_body_draws: null handle");
+    std::vector<int> cur;
+    std::vector<long long> cnt;
+    if (present_slots(h, h->env_body, 0, &cur, &cnt)) return 1;
+    const int n = h->n, nj = h->mc.nj;
+    std::vector<BodyConst> drawn;
+    if (h->ranges.body_ranged) {
+        drawn.resize((size_t)n);
+        CK(cudaMemcpy(drawn.data(), h->ranges.env_bdraw, (size_t)n * sizeof(BodyConst), cudaMemcpyDeviceToHost));
+    }
+    const BodyConst scene = body_of(h->mc);
+    for (int e = 0; e < n; ++e) {
+        const int b = cur[e];
+        const BodyConst& x = ((h->ranges.body_ranged >> b) & 1u) ? drawn[e] : (b == 0 ? scene : h->body[b]);
+        if (out) {
+            double* o = out + (size_t)e * kBodyDrawFields * nj;
+            for (int j = 0; j < nj; ++j) { o[j] = x.mass[j]; o[nj + j] = x.kp[j]; o[2 * nj + j] = x.kd[j]; o[3 * nj + j] = x.torque_lim[j]; }
+        }
+        if (draws) draws[e] = cnt[e];
+    }
+    return 0;
+}
+
+int trl_env_physics_draws(trl_handle* h, double* out, int64_t* draws) {
+    if (!h) return fail("trl_env_physics_draws: null handle");
+    std::vector<int> cur;
+    std::vector<long long> cnt;
+    if (present_slots(h, h->env_phys, 1, &cur, &cnt)) return 1;
+    const int n = h->n;
+    std::vector<PhysParams> drawn;
+    if (h->ranges.phys_ranged) {
+        drawn.resize((size_t)n);
+        CK(cudaMemcpy(drawn.data(), h->ranges.env_pdraw, (size_t)n * sizeof(PhysParams), cudaMemcpyDeviceToHost));
+    }
+    for (int e = 0; e < n; ++e) {
+        const int q = cur[e];
+        const PhysParams& x = ((h->ranges.phys_ranged >> q) & 1u) ? drawn[e] : (q == 0 ? h->mc.phys : h->phys[q]);
+        if (out) {
+            double* o = out + (size_t)e * 7;
+            o[0] = x.kn; o[1] = x.dn; o[2] = x.mu; o[3] = x.v_eps; o[4] = x.contact_tol; o[5] = x.k_lim; o[6] = x.d_lim;
+        }
+        if (draws) draws[e] = cnt[e];
+    }
+    return 0;
 }
 
 int trl_dist_log(trl_handle* h, const double** dist, const int32_t** env_id, int* n) {

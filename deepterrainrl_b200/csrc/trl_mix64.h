@@ -17,4 +17,24 @@ unsigned long long mix64(unsigned long long z) {
     return z ^ (z >> 31);
 }
 
+// The draws of ranged body and physics slots (trl_types.h: kBodyDrawTag).  Draw number `draw` of one kind (`tag`) of env `env` has
+// the key mix64(mix64(mix64(rng_seed ^ tag) + env) + draw); its i-th number is the top 53 bits of mix64(key + i), scaled into [0, 1)
+// (exact: a 53-bit integer times 2^-53).  The keys are their own, so a draw never moves the env's counter RNG.
+#if defined(__CUDACC__) && !defined(TRL_SIMT_EMU)
+__host__ __device__ __forceinline__
+#else
+inline
+#endif
+unsigned long long draw_key(unsigned long long rng_seed, unsigned long long tag, int env, long long draw) {
+    return mix64(mix64(mix64(rng_seed ^ tag) + (unsigned long long)env) + (unsigned long long)draw);
+}
+#if defined(__CUDACC__) && !defined(TRL_SIMT_EMU)
+__host__ __device__ __forceinline__
+#else
+inline
+#endif
+double draw_unit(unsigned long long key, int i) {
+    return (double)(mix64(key + (unsigned long long)i) >> 11) * 0x1.0p-53;
+}
+
 }  // namespace trl

@@ -32,6 +32,7 @@
 #include "trl_rcp.cuh"
 #include "trl_terrain.cuh"
 #include "trl_types.h"
+#include "trl_mix64.h"
 
 // The file is compiled twice: as is (namespace trl), and through trl_step_cg.cu with -Xptxas -dlcm=cg (namespace trl_cg), where
 // every global load bypasses L1.  The cg build serves the catch-up launches of the overlapped schedule: they read env state the
@@ -113,22 +114,30 @@ __device__ ModelConst g_model;
 #define TRL_LINK_SMEM 1     // 1: the per-lane link constants live in shared memory (one table per CTA) instead of ~28 registers per thread
                             //    (the register build spills them and reloads them inside the ABA rounds)
 #endif
-// Body slots: the per-link numbers of the env's body.  `bs` (the env's slot, warp-uniform: one env per warp) must be in scope.
-// BL: lane-indexed reads from the mirror g_body at the slot's base; BU: warp-uniform reads of a per-link number; BM: the slot's
-// total_mass / reach from constant memory (one broadcast).  The other builds read the scene's body from the model, as before slots.
-// The body build needs the link tables in shared memory (restaged per warp when its env changes body); the emulator's
-// TRL_LINK_SMEM=0 experiment build runs without body slots.
+// Body slots: the per-link numbers of the env's body.  `bb` (the env's body: its slot's entry of g_body, or on a ranged slot its own
+// drawn entry of c_env_bdraw; warp-uniform, one env per warp) must be in scope.  BL: lane-indexed reads; BU: warp-uniform reads of a
+// per-link number; BM: total_mass / reach.  They are coherent loads: a reset rewrites the drawn entry inside the launch that reads it.
+// The other builds read the scene's body from the model, as before slots.  The body build needs the link tables in shared memory
+// (restaged per warp when its env changes body); the emulator's TRL_LINK_SMEM=0 experiment build runs without body slots.
 #if (defined(TRL_BODY_SLOTS_VARIANT) || defined(TRL_SIMT_EMU)) && TRL_LINK_SMEM
 #define TRL_BODY_TABLE 1
-__device__ BodyConst g_body[kMaxBodySlots];      // slot 0 = the scene's body (trl_types.h: BodyConst)
-__constant__ double c_body_total_mass[kMaxBodySlots], c_body_reach[kMaxBodySlots];   // total_mass, reach of every slot
+__device__ BodyConst g_body[kMaxBodySlots];      // slot 0 = the scene's body; a ranged slot holds its lo numbers (trl_types.h: BodyConst)
+__device__ BodyConst g_body_hi[kMaxBodySlots];   // a ranged slot's hi numbers
 __constant__ int* c_env_body;                    // [2][n] of the owning handle: the body slot of every env's present episode, then the slot
                                                  // it gets at its next reset; null while the handle has no body slot
-#define BL(field, idx) __ldg(&g_body[bs].field[(idx)])
+// Ranged slots (trl_types.h: kBodyDrawTag): bit s of c_body_ranged / c_phys_ranged marks body / physics slot s as ranged.  The
+// per-env tables exist from the handle's first ranged slot on (null before): the drawn body and physics of every env's present
+// episode on a ranged slot, and every env's count of draws of either kind ([2][n]: body, physics)
+__constant__ unsigned c_body_ranged, c_phys_ranged;
+__constant__ PhysParams c_phys_hi[kMaxPhysSlots];
+__constant__ BodyConst* c_env_bdraw;
+__constant__ PhysParams* c_env_pdraw;
+__constant__ long long* c_env_draws;
+#define BL(field, idx) bb->field[(idx)]
 #define BU(field, idx) BL(field, idx)
-#define BM(field) c_body_##field[bs]
-#define TRL_BS_DECL , int bs
-#define TRL_BS_ARG , bs
+#define BM(field) bb->field
+#define TRL_BS_DECL , const BodyConst* bb
+#define TRL_BS_ARG , bb
 #else
 #if defined(TRL_BODY_SLOTS_VARIANT)
 #error "the body-slot build stages its link tables in shared memory (TRL_LINK_SMEM=1)"
@@ -246,8 +255,12 @@ __device__ unsigned long long g_phase_clocks[kNumPhases + 1];
 #else
 #define TRL_REUSE_KIN_DECL
 #endif
-// the physics slot of the env a sub-step serves (physics-slot builds only: the other builds keep the parent's signature)
-#if TRL_PHYS_TABLE
+// the physics slot of the env a sub-step serves (physics-slot builds only: the other builds keep the parent's signature); the body build
+// hands it the env's physics itself, staged per warp (a ranged slot's envs each have their own)
+#if TRL_BODY_TABLE
+#define TRL_PS_DECL , const PhysParams& pp
+#define TRL_PS_ARG , s_pp_w[warp]
+#elif TRL_PHYS_TABLE
 #define TRL_PS_DECL , int ps
 #define TRL_PS_ARG , ps
 #else
@@ -588,7 +601,7 @@ __device__ __forceinline__ void stage_link_tables(LinkTables* t TRL_BS_DECL) {
 #if TRL_BODY_TABLE
     {
         const int lane = threadIdx.x & 31;
-        const LinkVals v = link_values(lane, bs);
+        const LinkVals v = link_values(lane, bb);
 #else
     if (threadIdx.x < kWarp) {
         const int lane = threadIdx.x;
@@ -629,13 +642,13 @@ __device__ __forceinline__ LinkC load_link(int lane, const LinkTables* t) {
     return c;
 }
 #if TRL_BODY_TABLE
-// The warp's own tables for body slot bs: the link table, and (s_clx non-null) the corner tables with the six per-body box tables behind
+// The warp's own tables for body bb: the link table, and (s_clx non-null) the corner tables with the six per-body box tables behind
 // them (the layout the other builds stage once per CTA in trl_step_kernel).  The leading barrier lets every lane finish reading the tables
 // of the env's previous body; the trailing one publishes the new ones.
-__device__ __forceinline__ void stage_body(LinkTables* lt, double* s_clx, double* s_cly, int lane, int bs) {
+__device__ __forceinline__ void stage_body(LinkTables* lt, double* s_clx, double* s_cly, int lane, const BodyConst* bb) {
     const ModelConst& m = c_model;
     __syncwarp();
-    stage_link_tables(lt, bs);
+    stage_link_tables(lt, bb);
     if (s_clx) {
         for (int t = lane; t < m.n_corners; t += kWarp) { s_clx[t] = BL(corner_lx, t); s_cly[t] = BL(corner_ly, t); }
         if (lane < m.nj) {
@@ -647,16 +660,87 @@ __device__ __forceinline__ void stage_body(LinkTables* lt, double* s_clx, double
     }
     __syncwarp();
 }
-// at an episode reset: the body slot assigned to the env (trl_set_env_body) becomes its current one, and the warp restages its tables
-// for it.  Returns the slot
-__device__ __forceinline__ int begin_body(const Lane& L, LinkTables* lt, double* s_clx, double* s_cly, int lane) {
+// the draws run once per episode: out of line, they leave the step kernel's registers to its hot loop (inlined, its spill stores / loads
+// grow from 260 / 824 B to 324 / 1,276 B)
+#ifdef TRL_SIMT_EMU
+#define TRL_NOINLINE
+#else
+#define TRL_NOINLINE __noinline__
+#endif
+// one number of a ranged slot's draw (trl_types.h: kBodyDrawTag): lo + u (hi - lo), each operation rounded on its own, at most hi
+__device__ __forceinline__ double draw_in(double lo, double hi, double u) { return fmin(hi, __dadd_rn(lo, __dmul_rn(u, __dsub_rn(hi, lo)))); }
+// The env's body on ranged body slot bs for the episode a reset begins: the slot's table with Mass, Kp, Kd and TorqueLim drawn per link
+// (lane j draws link j), and izz_c, izz_o and total_mass derived from the drawn masses with fill_model's expressions (trl_host.cu), in
+// its association and each operation rounded on its own, so the entry equals what trl_load_body makes of a file holding the drawn
+// numbers.  Lane 0 sums total_mass over the links in index order, as fill_model does.  Writes the env's entry of c_env_bdraw.
+__device__ TRL_NOINLINE const BodyConst* draw_body(const Lane& L, int bs, int lane) {
+    const ModelConst& m = c_model;
+    BodyConst* d = c_env_bdraw + L.env;
+    const BodyConst& lo = g_body[bs];
+    const BodyConst& hi = g_body_hi[bs];
+    const unsigned long long* src = reinterpret_cast<const unsigned long long*>(&lo);
+    unsigned long long* dst = reinterpret_cast<unsigned long long*>(d);
+    static_assert(sizeof(BodyConst) % 8 == 0, "the body table is copied in 8-byte words");
+    for (int w = lane; w < (int)(sizeof(BodyConst) / 8); w += kWarp) dst[w] = src[w];
+    const long long draw = c_env_draws[L.env];
+    __syncwarp();
+    if (lane < m.nj) {
+        const int nj = m.nj;
+        const unsigned long long key = draw_key(m.rng_seed, kBodyDrawTag, L.env, draw);
+        const double mass = draw_in(lo.mass[lane], hi.mass[lane], draw_unit(key, lane));
+        d->mass[lane] = mass;
+        d->kp[lane] = draw_in(lo.kp[lane], hi.kp[lane], draw_unit(key, nj + lane));
+        d->kd[lane] = draw_in(lo.kd[lane], hi.kd[lane], draw_unit(key, 2 * nj + lane));
+        d->torque_lim[lane] = draw_in(lo.torque_lim[lane], hi.torque_lim[lane], draw_unit(key, 3 * nj + lane));
+        // the box sizes are twice the half sizes (exact), the centre offsets the BodyDefs AttachX / AttachY
+        const double sx = 2.0 * lo.half_x[lane], sy = 2.0 * lo.half_y[lane], ax = lo.body_ax[lane], ay = lo.body_ay[lane];
+        const double izz_c = __dmul_rn(__ddiv_rn(mass, 12.0), __dadd_rn(__dmul_rn(sx, sx), __dmul_rn(sy, sy)));
+        d->izz_c[lane] = izz_c;
+        d->izz_o[lane] = __dadd_rn(izz_c, __dmul_rn(mass, __dadd_rn(__dmul_rn(ax, ax), __dmul_rn(ay, ay))));
+    }
+    __syncwarp();
+    if (lane == 0) {
+        double total = 0.0;
+        for (int j = 0; j < m.nj; ++j) total = __dadd_rn(total, d->mass[j]);
+        d->total_mass = total;
+        c_env_draws[L.env] = draw + 1;
+    }
+    __syncwarp();
+    return d;
+}
+// The env's physics on ranged physics slot q for the episode a reset begins (lane 0): the seven constants drawn, vertex_contacts the slot's.
+// Writes the env's entry of c_env_pdraw
+__device__ TRL_NOINLINE void draw_phys(const Lane& L, int q) {
+    const long long draw = c_env_draws[(size_t)L.n + L.env];
+    const unsigned long long key = draw_key(c_model.rng_seed, kPhysDrawTag, L.env, draw);
+    const PhysParams& lo = c_phys[q];
+    const PhysParams& hi = c_phys_hi[q];
+    PhysParams* d = c_env_pdraw + L.env;
+    d->kn = draw_in(lo.kn, hi.kn, draw_unit(key, 0));
+    d->dn = draw_in(lo.dn, hi.dn, draw_unit(key, 1));
+    d->mu = draw_in(lo.mu, hi.mu, draw_unit(key, 2));
+    d->v_eps = draw_in(lo.v_eps, hi.v_eps, draw_unit(key, 3));
+    d->contact_tol = draw_in(lo.contact_tol, hi.contact_tol, draw_unit(key, 4));
+    d->k_lim = draw_in(lo.k_lim, hi.k_lim, draw_unit(key, 5));
+    d->d_lim = draw_in(lo.d_lim, hi.d_lim, draw_unit(key, 6));
+    d->vertex_contacts = lo.vertex_contacts;
+    c_env_draws[(size_t)L.n + L.env] = draw + 1;
+}
+// the body of the env's present episode: its slot's entry, or on a ranged slot its own drawn one
+__device__ __forceinline__ const BodyConst* env_body(int bs, int env) {
+    return ((c_body_ranged >> bs) & 1u) ? c_env_bdraw + env : &g_body[bs];
+}
+// at an episode reset: the body slot assigned to the env (trl_set_env_body) becomes its current one, a ranged slot draws the episode's
+// body, and the warp restages its tables for it.  Returns the body
+__device__ __forceinline__ const BodyConst* begin_body(const Lane& L, LinkTables* lt, double* s_clx, double* s_cly, int lane) {
     int bs = 0;
     if (c_env_body) {
         bs = c_env_body[(size_t)L.n + L.env];
         if (lane == 0) c_env_body[L.env] = bs;
     }
-    stage_body(lt, s_clx, s_cly, lane, bs);
-    return bs;
+    const BodyConst* bb = ((c_body_ranged >> bs) & 1u) ? draw_body(L, bs, lane) : &g_body[bs];
+    stage_body(lt, s_clx, s_cly, lane, bb);
+    return bb;
 }
 #endif
 
@@ -1134,7 +1218,9 @@ __device__ int physics_substep(const LinkC& lc, EnvRegs& e, const GroundView& g,
     const double *s_bax = s_clx + 4 * kMaxJoints, *s_bay = s_bax + kMaxJoints, *s_bc = s_bay + kMaxJoints, *s_bs = s_bc + kMaxJoints,
                  *s_hx = s_bs + kMaxJoints, *s_hy = s_hx + kMaxJoints;
     const ModelConst& m = c_model;
-#if TRL_PHYS_TABLE
+#if TRL_BODY_TABLE
+    // pp: the env's physics in the warp's shared-memory copy (the same in every lane: one broadcast per read)
+#elif TRL_PHYS_TABLE
     // the env's slot: ps is the same in every lane (one env per warp), so each read is one broadcast from the constant cache
     const PhysParams& pp = c_phys[ps];
 #else
@@ -1366,6 +1452,9 @@ __device__ void reset_env(Lane& L, const LinkC& lc, EnvRegs& e, const Buffers& B
         }
 #if TRL_PHYS_TABLE
         if (c_env_phys) c_env_phys[L.env] = c_env_phys[(size_t)L.n + L.env];   // likewise the physics slot (trl_set_env_physics)
+#if TRL_BODY_TABLE
+        if (c_env_phys && ((c_phys_ranged >> c_env_phys[L.env]) & 1u)) draw_phys(L, c_env_phys[L.env]);   // a ranged one draws
+#endif
         if (c_env_eval) {       // and the mode (trl_set_env_eval): evaluation counts cycles over episodes, from 0 when it begins
             const int next = c_env_eval[(size_t)L.n + L.env];
             if (next && !c_env_eval[L.env]) L.i(I_CYCLE_COUNT) = 0;
@@ -1423,9 +1512,10 @@ __device__ __forceinline__ void catchup_leave(const Buffers& B, int prev) {
 __global__ void __launch_bounds__(kBlockThreads, TRL_STEP_MIN_BLOCKS)
 trl_step_kernel(Buffers B, double h, int flags, int lists) {
 #if TRL_BODY_TABLE
-    // one copy of the link, corner and box tables per warp, staged below with its env's body
+    // one copy of the link, corner and box tables per warp, staged below with its env's body, and of the env's physics
     __shared__ double s_clx_w[kWarpsPerBlock][4 * kMaxJoints + 6 * kMaxJoints], s_cly_w[kWarpsPerBlock][4 * kMaxJoints];
     __shared__ LinkTables s_link_w[kWarpsPerBlock];
+    __shared__ PhysParams s_pp_w[kWarpsPerBlock];
 #else
     __shared__ double s_clx[4 * kMaxJoints + 6 * kMaxJoints], s_cly[4 * kMaxJoints];     // s_clx also carries the six per-body box tables
 #endif
@@ -1511,8 +1601,8 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
     }
     double* xs = s_x + warp * X_END;
 #if TRL_BODY_TABLE
-    int bs = c_env_body ? c_env_body[env] : 0;    // the body of the env's present episode; an episode reset below may change it
-    stage_body(link_tabs, s_clx, s_cly, lane, bs);
+    const BodyConst* bb = env_body(c_env_body ? c_env_body[env] : 0, env);   // the env's present body; an episode reset below may change it
+    stage_body(link_tabs, s_clx, s_cly, lane, bb);
 #endif
     const LinkC lc = load_link(lane, link_tabs);
     EnvRegs e;
@@ -1594,7 +1684,7 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
         }
         if (do_reset) {
 #if TRL_BODY_TABLE
-            bs = begin_body(L, link_tabs, s_clx, s_cly, lane);   // lc reads the warp's tables, which now hold the new episode's body
+            bb = begin_body(L, link_tabs, s_clx, s_cly, lane);   // lc reads the warp's tables, which now hold the new episode's body
 #endif
             reset_env(L, lc, e, B, lane TRL_RESET_XS_ARG TRL_BS_ARG); contact = 0;
 #if TRL_REUSE_KIN
@@ -1618,6 +1708,10 @@ trl_step_kernel(Buffers B, double h, int flags, int lists) {
 #if TRL_PHYS_TABLE
         // the slot of the env's present episode (a reset above has already made its assignment current)
         const int ps = c_env_phys ? c_env_phys[env] : 0;
+#endif
+#if TRL_BODY_TABLE
+        if (lane == 0) s_pp_w[warp] = ((c_phys_ranged >> ps) & 1u) ? c_env_pdraw[env] : c_phys[ps];
+        __syncwarp();
 #endif
 #if TRL_REUSE_KIN
         for (int s = 0; s < ns; ++s)
@@ -1739,7 +1833,7 @@ trl_reset_kernel(Buffers B, const uint64_t* terrain_seeds, const int* env_ids, i
     }
     __syncwarp();
 #if TRL_BODY_TABLE
-    const int bs = begin_body(L, link_tabs, nullptr, nullptr, lane);
+    const BodyConst* const bb = begin_body(L, link_tabs, nullptr, nullptr, lane);
 #endif
     const LinkC lc = load_link(lane, link_tabs);
     EnvRegs e;
@@ -1827,17 +1921,25 @@ cudaError_t upload_phys(const PhysParams* phys, int* env_phys, int* env_eval) {
 #if TRL_BODY_TABLE
 // the body table (slot 0 = the scene's body) and the handle's per-env slot array (null: every env on slot 0), uploaded with the model
 cudaError_t upload_body(const BodyConst* body, int* env_body) {
-    double tm[kMaxBodySlots], rc[kMaxBodySlots];
-    for (int s = 0; s < kMaxBodySlots; ++s) { tm[s] = body[s].total_mass; rc[s] = body[s].reach; }
     cudaError_t e = cudaMemcpyToSymbol(g_body, body, sizeof(BodyConst) * kMaxBodySlots);
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_body_total_mass, tm, sizeof(tm));
-    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_body_reach, rc, sizeof(rc));
     if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_body, &env_body, sizeof(env_body));
+    return e;
+}
+// the ranged slots (masks, hi tables) and the handle's per-env draw tables (null: the handle has no ranged slot), uploaded with the model
+cudaError_t upload_ranges(const RangeTables& r) {
+    cudaError_t e = cudaMemcpyToSymbol(g_body_hi, r.body_hi, sizeof(BodyConst) * kMaxBodySlots);
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_phys_hi, r.phys_hi, sizeof(PhysParams) * kMaxPhysSlots);
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_body_ranged, &r.body_ranged, sizeof(unsigned));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_phys_ranged, &r.phys_ranged, sizeof(unsigned));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_bdraw, &r.env_bdraw, sizeof(r.env_bdraw));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_pdraw, &r.env_pdraw, sizeof(r.env_pdraw));
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(c_env_draws, &r.env_draws, sizeof(r.env_draws));
     return e;
 }
 #elif defined(TRL_SIMT_EMU)
 // the emulator's TRL_LINK_SMEM=0 experiment build has no body slots: a handle with one is refused
 cudaError_t upload_body(const BodyConst*, int* env_body) { return env_body ? static_cast<cudaError_t>(1) : cudaSuccess; }
+cudaError_t upload_ranges(const RangeTables& r) { return r.env_draws ? static_cast<cudaError_t>(1) : cudaSuccess; }
 #endif
 size_t step_smem_bytes() { return 0; }
 // TRL_PHASE_CLOCKS builds: copy the accumulated phase clocks (kNumPhases + the env-step count) into out[], optionally zero them

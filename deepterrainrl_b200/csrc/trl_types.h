@@ -192,6 +192,29 @@ struct BodyConst {
 // reach about 1.1 m (dog, goat) and 1.0 m (raptor); trl_load_body refuses a reach above kMaxReach.
 constexpr double kMaxReach = 1.75;
 
+// Ranged slots (trl_load_body_range, trl_load_physics_range): a body or physics slot whose randomizable numbers are drawn again at
+// every episode reset of every env on it, each independently and uniformly in [lo, hi]:
+//   key = mix64(mix64(mix64(rng_seed ^ tag) + env) + draw)       tag: kBodyDrawTag or kPhysDrawTag; draw: the env's earlier draws of
+//                                                                that kind (from 0; carried by checkpoints, not reset by trl_reset)
+//   u_i = (mix64(key + i) >> 11) * 2^-53                         body: i = field * nj + link, fields Mass, Kp, Kd, TorqueLim;
+//                                                                physics: i = 0..6 in the order of PhysParams
+//   v_i = min(hi_i, lo_i + u_i * (hi_i - lo_i))                  every operation rounded on its own (no FMA); lo == hi gives lo
+// A body draw then derives izz_o, izz_c per link and total_mass (summed over the links from 0) with fill_model's expressions.  The
+// slot's table holds the lo numbers; everything but the drawn fields is the lo file's and equals the hi file's.
+constexpr unsigned long long kBodyDrawTag = 0x626f64792d726e67ull;   // "body-rng"
+constexpr unsigned long long kPhysDrawTag = 0x706879732d726e67ull;   // "phys-rng"
+constexpr int kBodyDrawFields = 4;
+// what the body-slot build holds of the ranged slots: their hi tables (the slot tables hold lo), which slots are ranged (bit s), and
+// the handle's per-env tables (trl_handle.h; null until its first ranged slot)
+struct RangeTables {
+    BodyConst body_hi[kMaxBodySlots];
+    PhysParams phys_hi[kMaxPhysSlots];
+    unsigned body_ranged, phys_ranged;
+    BodyConst* env_bdraw;        // [n] the drawn body of every env's present episode on a ranged body slot
+    PhysParams* env_pdraw;       // [n] likewise its drawn physics
+    long long* env_draws;        // [2][n] every env's draws so far: body, physics
+};
+
 // Exploration settings can change between updates (cScenarioExp::SetExpRate/Temp/BaseActionRate).
 struct ExpSettings {
     int enable;

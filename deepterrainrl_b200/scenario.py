@@ -142,6 +142,7 @@ EXPORTS = [
     "trl_load_physics", "trl_set_env_physics", "trl_env_physics", "trl_eval_stats_phys",
     "trl_set_env_eval", "trl_env_eval", "trl_eval_stats_mode",
     "trl_load_body", "trl_set_env_body", "trl_env_body", "trl_eval_stats_body",
+    "trl_load_body_range", "trl_load_physics_range", "trl_env_body_draws", "trl_env_physics_draws",
 ]
 
 
@@ -336,6 +337,36 @@ class BatchedScenario:
         nxt = np.zeros(self.num_envs, np.int32)
         self._ck(self.L.trl_env_body(self.h, _p(cur), _p(nxt), self.num_envs))
         return cur, nxt
+
+    def LoadBodyRange(self, slot, lo_path, hi_path):
+        """a ranged body slot 1..7 (domain randomization): at every episode reset of an env on it, each link's Mass, Kp, Kd and
+        TorqueLim are drawn uniformly between the lo and hi character files' values (include/terrainrl_b200.h gives the recipe).
+        Both files must pass LoadBody's checks and agree in everything else.  Envs move to it with SetEnvBody."""
+        self._ck(self.L.trl_load_body_range(self.h, int(slot), os.fspath(lo_path).encode(), os.fspath(hi_path).encode()))
+
+    def LoadPhysicsRange(self, slot, lo7, hi7, vertex_contacts=False):
+        """a ranged physics slot 1..7: at every episode reset of an env on it, each of the seven constants (LoadPhysics order) is drawn
+        uniformly in [lo7[k], hi7[k]].  Envs move to it with SetEnvPhysics."""
+        lo = np.ascontiguousarray(lo7, dtype=np.float64).ravel()
+        hi = np.ascontiguousarray(hi7, dtype=np.float64).ravel()
+        if lo.size != 7 or hi.size != 7:
+            raise ValueError("LoadPhysicsRange: 7 parameters at each end")
+        self._ck(self.L.trl_load_physics_range(self.h, int(slot), _p(lo), _p(hi), int(bool(vertex_contacts))))
+
+    def EnvBodyDraws(self):
+        """(numbers [n][4][nj]: Mass, Kp, Kd, TorqueLim of every env's present episode; draws [n]: its body draws so far).  An env on a
+        fixed body slot reports its slot's numbers."""
+        out = np.zeros((self.num_envs, 4, self.num_joints), np.float64)
+        draws = np.zeros(self.num_envs, np.int64)
+        self._ck(self.L.trl_env_body_draws(self.h, _p(out), _p(draws)))
+        return out, draws
+
+    def EnvPhysicsDraws(self):
+        """(numbers [n][7] of every env's present episode in LoadPhysics order; draws [n]: its physics draws so far)"""
+        out = np.zeros((self.num_envs, 7), np.float64)
+        draws = np.zeros(self.num_envs, np.int64)
+        self._ck(self.L.trl_env_physics_draws(self.h, _p(out), _p(draws)))
+        return out, draws
 
     def SetEnvEval(self, flags, env_ids=None):
         """env_ids[k] (default: env k) of an exploration scenario evaluates its policy slot's current net, exploration off and no

@@ -273,6 +273,36 @@ int trl_set_env_body(trl_handle* h, const int32_t* env_ids, const int32_t* slots
 int trl_env_body(trl_handle* h, int32_t* current, int32_t* assigned, int n);
 int trl_eval_stats_body(trl_handle* h, int mode, int policy_slot, int terrain_slot, int phys_slot, int body_slot, int64_t* cycles,
                         int64_t* episodes, double* avg_dist, int64_t* env_steps);
+/* Ranged slots (domain randomization; any mode): a body or physics slot whose randomizable numbers are drawn again at every episode
+ * reset of every env on it (a fall inside trl_update, trl_reset, trl_seed_terrain).  With the same seeds, an episode of env i on a
+ * ranged slot computes bit for bit what env i computes on a fixed slot loaded with that episode's drawn numbers (a character file
+ * holding them for trl_load_body, the drawn p7 for trl_load_physics), and so what a handle created with that file / those constants
+ * computes.  The draws have keys of their own and never move an env's counter RNG.  Each number is drawn independently:
+ *   key  = mix64(mix64(mix64(rng_seed ^ TAG) + env) + draw)   mix64: the splitmix64 finaliser; rng_seed: the handle's seed; env: the
+ *                                                             env's index; draw: the env's earlier draws of that kind (from 0; kept
+ *                                                             by checkpoints, not reset by trl_reset or trl_seed_terrain);
+ *                                                             TAG = 0x626f64792d726e67 for bodies, 0x706879732d726e67 for physics
+ *   u_i  = (mix64(key + i) >> 11) * 2^-53                     body: i = field * nj + link, fields Mass, Kp, Kd, TorqueLim;
+ *                                                             physics: i = 0..6 in p7 order
+ *   v_i  = min(hi_i, lo_i + u_i * (hi_i - lo_i))              each operation rounded on its own; lo == hi gives lo exactly
+ * A body draw derives izz (per link) and the total mass from the drawn masses as trl_load_body does.  The root's Kp and Kd stay 0.
+ *   trl_load_body_range      lo and hi character files into slot 1..7: per link Mass, Kp, Kd and TorqueLim are drawn; everything else is
+ *                            the files' and must be the same in both.  Refused, handle unchanged, for whatever trl_load_body refuses
+ *                            in either file, two files that differ in anything but the four drawn fields (the message names the
+ *                            field and link), lo > hi in any of them, and a handle with a communicator.
+ *   trl_load_physics_range   lo7 and hi7 (kn, dn, mu, v_eps, contact_tol, k_lim, d_lim) into slot 1..7, vertex_contacts fixed.
+ *                            Refused, handle unchanged, when either end fails trl_load_physics's checks, lo > hi in any constant, the
+ *                            slot is some env's present or assigned physics, or the handle has a communicator.
+ * Envs move onto ranged slots with trl_set_env_body / trl_set_env_physics; to trl_env_body, the statistics entries and the Python
+ * filters a ranged slot is a slot.  trl_load_body / trl_load_physics make a slot fixed again.  The first ranged slot allocates the
+ * per-env tables (about 4.7 KB per env) and moves the handle onto the body-slot build.
+ *   trl_env_body_draws       the numbers of every env's present episode: out[n][4][nj] (Mass, Kp, Kd, TorqueLim), draws[n] its body
+ *                            draws so far; an env on a fixed slot reports its slot's numbers.  Either pointer may be NULL.
+ *   trl_env_physics_draws    likewise out[n][7] (p7 order) and draws[n] of physics. */
+int trl_load_body_range(trl_handle* h, int slot, const char* lo_path, const char* hi_path);
+int trl_load_physics_range(trl_handle* h, int slot, const double* lo7, const double* hi7, int vertex_contacts);
+int trl_env_body_draws(trl_handle* h, double* out, int64_t* draws);
+int trl_env_physics_draws(trl_handle* h, double* out, int64_t* draws);
 int trl_pack_output_offset_scale(const char* pack_path, double* offset, double* scale, int n_out);   /* host only, no device */
 
 /* cScenarioSimChar::SetTerrainParamsLerp (scenarios/ScenarioSimChar.cpp:255-272) and cScenarioTrain's annealing schedule
