@@ -94,10 +94,11 @@ int nccl_fail(const char* what, int rc) {
 namespace trl_comm_k {
 
 // Pack the rank's tuple block for the exchange.  One CTA per tuple slot; slots [0, m) go to the send block as
-// {flags (bit 31 = failed cNeuralNetTrainer::CheckTuple, evaluated on the f64 values), env_offset + env, f32 row}; slots
-// [m, count) -- more tuples than one block carries -- go to the scratch block and are moved to the front by k_pack_finish.
+// {flags (bit 31 = failed cNeuralNetTrainer::CheckTuple, evaluated on the f64 values; bits 24..26 = the env's policy slot when
+// env_slot is given, i.e. in a handle with training slots), env_offset + env, f32 row}; slots [m, count) -- more tuples than one
+// block carries -- go to the scratch block and are moved to the front by k_pack_finish.
 __global__ void k_pack_tuples(Buffers B, unsigned char* send, int R, int W, int rank, long long env_offset, double* scr_rows,
-                              uint32_t* scr_flags, int* scr_env, int* dropped) {
+                              uint32_t* scr_flags, int* scr_env, int* dropped, const int* env_slot) {
     const int raw = *B.tuple_count;
     const int count = min(raw, B.tuple_cap);
     const int m = min(count, R);
@@ -117,8 +118,10 @@ __global__ void k_pack_tuples(Buffers B, unsigned char* send, int R, int W, int 
         for (int k = threadIdx.x; k < W; k += blockDim.x) { const double v = src[k]; bad |= !isfinite(v); rows[k] = (float)v; }
         bad = __syncthreads_or(bad);
         if (threadIdx.x == 0) {
-            flags[i] = (B.tuple_flags[i] & 0x7fffffffu) | (bad ? 0x80000000u : 0u);
-            env[i] = (int)(env_offset + B.tuple_env[i]);
+            const int e = B.tuple_env[i];
+            const uint32_t slot = env_slot ? (uint32_t)env_slot[e] << 24 : 0u;
+            flags[i] = (B.tuple_flags[i] & 0x7fffffffu) | slot | (bad ? 0x80000000u : 0u);
+            env[i] = (int)(env_offset + e);
         }
     } else {
         double* dst = scr_rows + (size_t)(i - m) * W;
@@ -163,7 +166,6 @@ struct trl_comm {
     trl_collectives coll{};
     cudaStream_t stream = nullptr;        // collectives run here; ordered against the handle's stream with events
     cudaEvent_t ev_packed = nullptr, ev_gathered = nullptr, ev_misc = nullptr, ev_consumed = nullptr;
-    bool consumed_pending = false;        // a consumer on another stream has yet to finish reading recv (trl_comm_mark_consumed)
     int block_rows = 0, width = 0;
     size_t block_bytes = 0;
     unsigned char *send = nullptr, *recv = nullptr;
@@ -171,7 +173,7 @@ struct trl_comm {
     uint32_t* scr_flags = nullptr;
     int* scr_env = nullptr;
     int* dropped = nullptr;               // device counter
-    double* small = nullptr;              // [8] device scratch for the small reductions
+    double* small = nullptr;              // [9] device scratch for the small reductions
     double* wscratch = nullptr;           // parameter-sized scratch (replica check)
     size_t wscratch_n = 0;
     long long env_offset = 0;
@@ -210,10 +212,14 @@ static int group_end(trl_comm* c) {
     return rc ? nccl_fail("ncclGroupEnd", rc) : 0;
 }
 
+// cudaMemset of device memory runs on the legacy default stream, which does not order against the handle's non-blocking streams:
+// without the synchronisation a late memset could clear what the first kernel or copy on those streams wrote (the replica check's
+// scratch, a first send block)
 template <typename T>
 static cudaError_t calloc_dev(trl_comm* c, T** p, size_t count) {
     cudaError_t e = cudaMalloc((void**)p, std::max<size_t>(count, 1) * sizeof(T));
     if (e == cudaSuccess) { c->allocs.push_back(*p); e = cudaMemset(*p, 0, std::max<size_t>(count, 1) * sizeof(T)); }
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
     return e;
 }
 
@@ -227,7 +233,7 @@ static int comm_common(trl_handle* h, trl_comm* c) {
     c->width = 1 + h->B.S + h->B.A + h->B.S;
     c->env_offset = (long long)c->rank * h->n;
     CCK(calloc_dev(c, &c->dropped, 1));
-    CCK(calloc_dev(c, &c->small, 8));
+    CCK(calloc_dev(c, &c->small, 9));
     CCK(calloc_dev(c, &c->scr_rows, (size_t)h->B.tuple_cap * c->width));
     CCK(calloc_dev(c, &c->scr_flags, (size_t)h->B.tuple_cap));
     CCK(calloc_dev(c, &c->scr_env, (size_t)h->B.tuple_cap));
@@ -339,14 +345,13 @@ int trl_gather_tuples(trl_handle* h, int block_rows) {
     if (c->gathered) CCK(cudaStreamWaitEvent(h->stream, c->ev_gathered, 0));
     const Buffers& B = h->B;
     TRL_LAUNCH(trl_comm_k::k_pack_tuples, B.tuple_cap, 128, 0, h->stream, B, c->send, c->block_rows, c->width, c->rank, c->env_offset,
-               c->scr_rows, c->scr_flags, c->scr_env, c->dropped);
+               c->scr_rows, c->scr_flags, c->scr_env, c->dropped, h->train_slots ? h->P.env_slot : (const int*)nullptr);
     TRL_LAUNCH(trl_comm_k::k_pack_finish, B.tuple_cap, 128, 0, h->stream, B, (const unsigned char*)c->send, c->width,
                (const double*)c->scr_rows, (const uint32_t*)c->scr_flags, (const int*)c->scr_env);
     h->launches += 2;
     CCK(cudaGetLastError());
     CCK(cudaEventRecord(c->ev_packed, h->stream));
     CCK(cudaStreamWaitEvent(c->stream, c->ev_packed, 0));
-    if (c->consumed_pending) { CCK(cudaStreamWaitEvent(c->stream, c->ev_consumed, 0)); c->consumed_pending = false; }
     if (coll_all_gather(c, c->send, c->recv, c->block_bytes)) return 1;
     CCK(cudaEventRecord(c->ev_gathered, c->stream));
     c->gathered = true;
@@ -462,6 +467,24 @@ int trl_comm_eval_stats(trl_handle* h, int64_t* cycles, int64_t* episodes, doubl
     return 0;
 }
 
+// trl_comm_eval_stats over the envs of one policy slot: trl_eval_stats_slot of every rank, summed
+int trl_comm_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps) {
+    if (!h || !h->comm) return trl_fail("trl_comm_eval_stats_slot: no communicator (trl_comm_init first)");
+    trl_comm* c = h->comm;
+    if (trl_slot_stats_dev(h, "trl_comm_eval_stats_slot", slot, c->small)) return 1;
+    CCK(cudaEventRecord(c->ev_misc, h->stream));
+    CCK(cudaStreamWaitEvent(c->stream, c->ev_misc, 0));
+    if (coll_all_reduce_sum(c, c->small, 4)) return 1;
+    CCK(cudaStreamSynchronize(c->stream));
+    double st[4];
+    CCK(cudaMemcpy(st, c->small, 32, cudaMemcpyDeviceToHost));
+    if (cycles) *cycles = (int64_t)st[0];
+    if (episodes) *episodes = (int64_t)st[1];
+    if (env_steps) *env_steps = (int64_t)st[2];
+    if (avg_dist) *avg_dist = st[1] > 0 ? st[3] / st[1] : 0.0;
+    return 0;
+}
+
 }  // extern "C"
 
 // ---------------------------------------------------------------------------------------------------- used by trl_train.cu
@@ -483,10 +506,12 @@ int trl_comm_view_on(trl_handle* h, trl_comm_blocks* out, cudaStream_t consumer)
     out->world = c->world; out->rank = c->rank;
     return 0;
 }
+// the comm stream waits for every consumer as it is marked (a join): any number of trainers, each on its own stream, may read one
+// gathered set of blocks, and the next all-gather overwrites them only after the last of them
 int trl_comm_mark_consumed(trl_handle* h, cudaStream_t consumer) {
     if (!h || !h->comm) return 0;
     CCK(cudaEventRecord(h->comm->ev_consumed, consumer));
-    h->comm->consumed_pending = true;
+    CCK(cudaStreamWaitEvent(h->comm->stream, h->comm->ev_consumed, 0));
     return 0;
 }
 int trl_comm_broadcast_list(trl_handle* h, double* const* arrays, const size_t* counts, int n, int root) {
@@ -510,5 +535,28 @@ int trl_comm_replica_spread(trl_handle* h, const double* theta, size_t n, double
     if (coll_all_reduce_sum(c, c->small + 4, 1)) return 1;
     CCK(cudaStreamSynchronize(c->stream));
     CCK(cudaMemcpy(out, c->small + 4, 8, cudaMemcpyDeviceToHost));
+    return 0;
+}
+// Do all ranks hold the same 64-bit signature, and did every rank accept the call (`ok`)?  Four 16-bit pieces v, their squares and a
+// refusal count go through one all-reduce; the pieces agree on every rank iff (sum v)^2 == world * sum v^2 (Cauchy-Schwarz), and every
+// rank evaluates that on the same reduced numbers, so all ranks reach the same answers.  The sums stay below 2^53, exact in f64, up to
+// 1024 ranks.  Synchronises.
+int trl_comm_agree(trl_handle* h, uint64_t sig, bool ok, bool* same, bool* all_ok) {
+    if (!h || !h->comm) return trl_fail("trainer: the scenario has no communicator (trl_comm_init first)");
+    trl_comm* c = h->comm;
+    double v[9];
+    for (int k = 0; k < 4; ++k) {
+        v[k] = (double)((sig >> (16 * k)) & 0xffffu);
+        v[4 + k] = v[k] * v[k];
+    }
+    v[8] = ok ? 0.0 : 1.0;
+    CCK(cudaStreamSynchronize(h->stream));
+    CCK(cudaMemcpyAsync(c->small, v, sizeof(v), cudaMemcpyHostToDevice, c->stream));
+    if (coll_all_reduce_sum(c, c->small, 9)) return 1;
+    CCK(cudaMemcpyAsync(v, c->small, sizeof(v), cudaMemcpyDeviceToHost, c->stream));
+    CCK(cudaStreamSynchronize(c->stream));
+    *same = true;
+    for (int k = 0; k < 4; ++k) *same = *same && v[k] * v[k] == (double)c->world * v[4 + k];
+    *all_ok = v[8] == 0.0;
     return 0;
 }

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <cstddef>
+#include <cstdint>
 
 struct trl_handle;
 
@@ -21,3 +22,8 @@ int trl_comm_replica_spread(trl_handle* h, const double* theta, size_t n, double
 // the next all-gather wait until `mark_consumed` has been recorded on that stream
 int trl_comm_view_on(trl_handle* h, trl_comm_blocks* out, cudaStream_t consumer);
 int trl_comm_mark_consumed(trl_handle* h, cudaStream_t consumer);
+// whether every rank passed the same signature, and whether every rank passed ok (one small all-reduce; synchronises).  Every rank
+// gets the same answers.
+int trl_comm_agree(trl_handle* h, uint64_t sig, bool ok, bool* same, bool* all_ok);
+// policy slot `slot`'s {cycles, episodes, env-steps, distance sum} into device memory out4 on the handle's stream (trl_host.cu)
+extern "C" int trl_slot_stats_dev(trl_handle* h, const char* who, int slot, double* out4);

@@ -1543,6 +1543,23 @@ int trl_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episo
     return eval_stats_cell(h, "trl_eval_stats_slot", slot, -1, cycles, episodes, avg_dist, env_steps);
 }
 
+// policy slot `slot`'s statistics as trl_eval_stats_slot counts them, {cycles, episodes, env-steps, distance sum}, into device memory
+// out4 on the handle's stream: the operand of the all-reduce of trl_comm_eval_stats_slot
+int trl_slot_stats_dev(trl_handle* h, const char* who, int slot, double* out4) {
+    if (slot < 0 || slot >= kMaxPolicySlots) return fail(std::string(who) + ": slot " + std::to_string(slot) + " out of range");
+    if (!slot_loaded(h, slot)) return fail(std::string(who) + ": policy slot " + std::to_string(slot) + " is empty");
+    if (!h->slots_active) {
+        launch_stats(h->B, out4, h->stream);
+    } else {
+        if (!h->cell_stats) CK(dalloc(h, &h->cell_stats, (size_t)(kMaxPolicySlots + 1) * (kMaxTerrainSlots + 1) * 4));
+        launch_cell_stats(h->B, h->P.env_slot, h->cell_stats, h->stream);
+        CK(cudaMemcpyAsync(out4, h->cell_stats + 4 * (slot * (kMaxTerrainSlots + 1) + kMaxTerrainSlots), 32, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->launches += 1;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 static bool phys_loaded(const trl_handle* h, int slot) { return slot == 0 || (slot > 0 && slot < kMaxPhysSlots && h->phys_loaded[slot]); }
 
 // physics slot `slot` >= 1 holds `q` (its numbers checked), fixed or (hi non-null) ranged up to *hi, and the handle moves onto the

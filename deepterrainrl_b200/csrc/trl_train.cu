@@ -386,17 +386,24 @@ __device__ __forceinline__ const int* gb_hdr(const GBlocks& g, int r) { return (
 __device__ __forceinline__ const uint32_t* gb_flags(const GBlocks& g, int r) { return (const uint32_t*)(g.recv + (size_t)r * g.block_bytes + 16); }
 __device__ __forceinline__ const int* gb_env(const GBlocks& g, int r) { return (const int*)(g.recv + (size_t)r * g.block_bytes + 16 + (size_t)4 * g.R); }
 __device__ __forceinline__ const float* gb_rows(const GBlocks& g, int r) { return (const float*)(g.recv + (size_t)r * g.block_bytes + 16 + (size_t)8 * g.R); }
+// In a handle with training slots the gathered intake of trainer `slot` takes only the rows whose flag bits 24..26 name its slot
+// (kSlot): they are ranked first inside each block, by env id, the other rows after them; those are invalid and take no replay slot,
+// so the replay memory sees what a single trainer fed only this slot's rows (rank order, env order inside a rank) sees.  The plain
+// order and copy kernels are the kSlot = false instances (their SASS is the one they had as plain kernels).
+__device__ __forceinline__ bool gb_mine(uint32_t f, int slot) { return (int)((f >> 24) & 7u) == slot; }
 // grid (R, world): rank of tuple j inside its block by env id -> d.order[r * R + rank_in_block] = j
-__global__ void k_addg_order(Dev d, GBlocks g) {
+template <bool kSlot>
+__device__ __forceinline__ void addg_order(const Dev& d, const GBlocks& g, int slot) {
     pdl_sync();
     const int r = blockIdx.y, i = blockIdx.x;
     const int count = min(max(gb_hdr(g, r)[0], 0), g.R);
     if (i >= count) return;
     const int* env = gb_env(g, r);
-    const int key = env[i];
+    const uint32_t* fl = gb_flags(g, r);
+    const int key = kSlot ? env[i] | (gb_mine(fl[i], slot) ? 0 : 0x40000000) : env[i];
     int rk = 0;
     for (int j = threadIdx.x; j < count; j += blockDim.x) {
-        const int kj = env[j];
+        const int kj = kSlot ? env[j] | (gb_mine(fl[j], slot) ? 0 : 0x40000000) : env[j];
         rk += (kj < key) || (kj == key && j < i);
     }
     __shared__ int red[32];
@@ -436,7 +443,36 @@ __global__ void k_addg_assign(Dev d, GBlocks g) {
         gc.add_count = total;
     }
 }
-__global__ void k_addg_copy(Dev d, GBlocks g) {
+// k_addg_assign with the slot filter, written out rather than shared: as one template the plain instance compiled to other SASS
+__global__ void k_addg_assign_slot(Dev d, GBlocks g, int slot) {
+    pdl_sync();
+    if (blockIdx.x != 0 || threadIdx.x >= 32) return;
+    const int lane = threadIdx.x;
+    Counters c = *d.c;
+    int total = 0;
+    for (int r = 0; r < g.world; ++r) {
+        const int count = min(max(gb_hdr(g, r)[0], 0), g.R);
+        const uint32_t* flags = gb_flags(g, r);
+        for (int base = 0; base < count; base += 32) {
+            const int k = base + lane;
+            const bool in = k < count;
+            const int j = in ? d.order[r * g.R + k] : 0;
+            const uint32_t f = in ? flags[j] : 0x80000000u;
+            const bool take = in && !(f & 0x80000000u) && gb_mine(f, slot);
+            const int t = assign_batch(d, c, take, f);
+            if (in) d.slot[r * g.R + j] = t;
+        }
+        total += count;
+    }
+    if (lane == 0) {
+        Counters& gc = *d.c;
+        gc.head = c.head; gc.num = c.num; gc.total = c.total; gc.actor_count = c.actor_count; gc.critic_count = c.critic_count;
+        gc.actor_batch_count = c.actor_batch_count;
+        gc.add_count = total;
+    }
+}
+template <bool kSlot>
+__device__ __forceinline__ void addg_copy(const Dev& d, const GBlocks& g) {
     pdl_sync();
     const int r = blockIdx.y, j = blockIdx.x;
     const int count = min(max(gb_hdr(g, r)[0], 0), g.R);
@@ -446,8 +482,12 @@ __global__ void k_addg_copy(Dev d, GBlocks g) {
     const float* src = gb_rows(g, r) + (size_t)j * d.Wd;
     float* dst = d.mem + (size_t)t * d.Wd;
     for (int k = threadIdx.x; k < d.Wd; k += blockDim.x) dst[k] = src[k];
-    if (threadIdx.x == 0) d.flags[t] = (int)(gb_flags(g, r)[j] & 0x7fffffffu);
+    if (threadIdx.x == 0) d.flags[t] = (int)(gb_flags(g, r)[j] & (kSlot ? 0x00ffffffu : 0x7fffffffu));
 }
+__global__ void k_addg_order(Dev d, GBlocks g) { addg_order<false>(d, g, 0); }
+__global__ void k_addg_copy(Dev d, GBlocks g) { addg_copy<false>(d, g); }
+__global__ void k_addg_order_slot(Dev d, GBlocks g, int slot) { addg_order<true>(d, g, slot); }
+__global__ void k_addg_copy_slot(Dev d, GBlocks g) { addg_copy<true>(d, g); }
 
 // ================================================================================================ stage switch
 __global__ void k_stage_check(Dev d) {
@@ -1085,7 +1125,6 @@ trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* p, c
         if (h->mode != TRL_MODE_EXPLORE) return refuse("trl_trainer_create_slot: training slots are for exploration handles (TRL_MODE_EXPLORE)");
         if (h->slot_trainer[slot]) return refuse("trl_trainer_create_slot: slot " + std::to_string(slot) + " already has a trainer");
         if (!h->decide_v2) return refuse("trl_trainer_create_slot: the TRL_DECIDE_V1 decision kernel has no policy slots");
-        if (h->comm) return refuse("trl_trainer_create_slot: training slots do not exchange tuples between GPUs (the handle has a communicator)");
     }
     trl_trainer* t = trainer_new(h, p);
     if (!t) return nullptr;
@@ -1207,14 +1246,13 @@ int trl_trainer_add_device(trl_trainer* t, const double* rows_dev, const uint32_
     return 0;
 }
 
-// AddTuples of the blocks every rank contributed to the last trl_gather_tuples (rank order, env order inside a rank), on the
-// scenario's stream behind the all-gather; identical input on every rank keeps replicated trainers bit-identical
-int trl_trainer_add_gathered(trl_trainer* t) {
-    TRL_TRAINER_LIVE(t);
+// AddTuples of the blocks every rank contributed to the last trl_gather_tuples (rank order, env order inside a rank), on stream `ws`
+// behind the all-gather; identical input on every rank keeps replicated trainers bit-identical.  In a handle with training slots the
+// trainer takes only its slot's rows (the pack kernel stamped each row with its env's slot)
+static int add_gathered_on(trl_trainer* t, cudaStream_t ws) {
     trl_handle* h = t->h;
     trl_comm_blocks v;
-    cudaStream_t ws = t->work();
-    if (t->async ? trl_comm_view_on(h, &v, ws) : trl_comm_view(h, &v)) return 1;
+    if (ws == h->stream ? trl_comm_view(h, &v) : trl_comm_view_on(h, &v, ws)) return 1;
     if (v.width != t->d.Wd) return trl_fail("trl_trainer_add_gathered: tuple width mismatch");
     if ((long long)v.world * v.block_rows > t->gather_cap) {
         // valid / slot / order are indexed by rank * block_rows + j
@@ -1223,17 +1261,30 @@ int trl_trainer_add_gathered(trl_trainer* t) {
         TCK(cudaStreamSynchronize(h->stream));
         TCK(cudaStreamSynchronize(ws));
         TCK(talloc(t, &nv, need)); TCK(talloc(t, &ns, need)); TCK(talloc(t, &no, need));
+        TCK(cudaDeviceSynchronize());      // talloc's memsets run on the legacy stream: done before the intake kernels on `ws` write
         t->d.valid = nv; t->d.slot = ns; t->d.order = no;
         t->gather_cap = (long long)need;
     }
     const Dev& d = t->d;
     const GBlocks g{v.recv, v.block_bytes, v.block_rows, v.world};
-    launch_pdl(k_addg_order, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g);
-    launch_pdl(k_addg_assign, dim3(1), dim3(32), 0, ws, d, g);
-    launch_pdl(k_addg_copy, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g);
+    if (h->train_slots) {
+        launch_pdl(k_addg_order_slot, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g, t->slot);
+        launch_pdl(k_addg_assign_slot, dim3(1), dim3(32), 0, ws, d, g, t->slot);
+        launch_pdl(k_addg_copy_slot, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g);
+    } else {
+        launch_pdl(k_addg_order, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g);
+        launch_pdl(k_addg_assign, dim3(1), dim3(32), 0, ws, d, g);
+        launch_pdl(k_addg_copy, dim3(v.block_rows, v.world), dim3(128), 0, ws, d, g);
+    }
     t->launches += 3;
     TCK(cudaGetLastError());
-    if (t->async && trl_comm_mark_consumed(h, ws)) return 1;      // the next all-gather may overwrite the blocks only after this
+    return 0;
+}
+int trl_trainer_add_gathered(trl_trainer* t) {
+    TRL_TRAINER_LIVE(t);
+    cudaStream_t ws = t->work();
+    if (add_gathered_on(t, ws)) return 1;
+    if (t->async && trl_comm_mark_consumed(t->h, ws)) return 1;      // the next all-gather may overwrite the blocks only after this
     return 0;
 }
 
@@ -1342,7 +1393,8 @@ int trl_trainer_set_async(trl_trainer* t, int enable) {
     TRL_TRAINER_LIVE(t);
     trl_handle* h = t->h;
     if ((enable != 0) == t->async) return 0;
-    if (h->train_slots) return trl_fail("trl_trainer_set_async: the handle has training slots (their trainers run in lock-step: trl_train_run_slots)");
+    if (h->train_slots && !h->comm)
+        return trl_fail("trl_trainer_set_async: the handle has training slots and no communicator (asynchronous slot trainers run through trl_train_run_slots_comm)");
     TCK(trainer_sync(t));
     const Dev& d = t->d;
     if (t->train_graph) { cudaGraphExecDestroy(t->train_graph); t->train_graph = nullptr; }      // it was captured on the other stream
@@ -1365,12 +1417,19 @@ int trl_trainer_set_async(trl_trainer* t, int enable) {
         TCK(cudaMemcpy(sn + d.P + 2 * d.S, d.out_off, (size_t)d.n_out * 8, cudaMemcpyDeviceToDevice));
         TCK(cudaMemcpy(sn + d.P + 2 * d.S + d.n_out, d.out_scale, (size_t)d.n_out * 8, cudaMemcpyDeviceToDevice));
     }
-    // bind the decision kernels to the snapshot (async) or straight to the trainer's arrays (synchronous: SyncNet as a pointer binding)
+    // bind the decision kernels to the snapshot (async) or straight to the trainer's arrays (synchronous: SyncNet as a pointer binding);
+    // a training slot's net through its entry of the slot table (and its terr_ip0 descriptor), rewritten before the next decision
     const double* th = enable ? t->snap : d.theta;
     const double* blobs[26];
     for (int b = 0; b < 26; ++b) blobs[b] = th + d.off[b];
-    h->W = net_weights(blobs, enable ? t->snap + d.P : d.in_off, enable ? t->snap + d.P + d.S : d.in_scale,
-                       enable ? t->snap + d.P + 2 * d.S : d.out_off, enable ? t->snap + d.P + 2 * d.S + d.n_out : d.out_scale);
+    const NetWeights nw = net_weights(blobs, enable ? t->snap + d.P : d.in_off, enable ? t->snap + d.P + d.S : d.in_scale,
+                                      enable ? t->snap + d.P + 2 * d.S : d.out_off, enable ? t->snap + d.P + 2 * d.S + d.n_out : d.out_scale);
+    if (t->slot == 0) {
+        h->W = nw;
+    } else {
+        h->slot_W[t->slot] = nw;
+        h->slot_dirty = true;
+    }
     trl_drop_graphs(h);
     t->async = enable != 0;
     t->trained_pending = t->job_pending = false;
@@ -1497,10 +1556,17 @@ int trl_train_run_timed(trl_trainer* t, const double* sp, int num_updates, int i
 //   iters_per_update == 0: train_run_impl's pacing per trainer: the schedule at the trainer's iteration counter at the start of the
 //   update, then k_i = (fresh tuples + carry) / tuple_buffer_size iterations.  The counters of all k trainers come back in one round
 //   trip at the start of the update and one after the hand-overs, so the iterations need a second fork behind the first join.
+//   comm = true (trl_train_run_slots_comm): the update is followed by ONE trl_gather_tuples(h, block_rows) and each branch takes its
+//   slot's rows of the gathered blocks instead (rank order, env order inside a rank); the pack kernel clears the block, keeping the
+//   rows beyond block_rows queued.  Every rank sees the same blocks, so counters, pacing and replicas agree across ranks.
+//   Asynchronous trainers (comm only, all or none, lock-step): per update each trainer's async_turnover -- wait for its previous
+//   job, refresh its snapshot, enqueue its intake of the last gathered blocks and its iterations on its own async stream --, then the
+//   update and the gather.  The next all-gather waits for every trainer's intake (trl_comm_mark_consumed joins the consumers).
 // The caller has checked the curricula: every trainer sees the same phase at every update, so the blend is trainer 0's.
 static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const double* sp, bool per_slot, int num_updates,
-                          int iters_per_update, int tuple_buffer_size, double time_step) {
+                          int iters_per_update, int tuple_buffer_size, double time_step, bool comm = false, int block_rows = 0) {
     trl_handle* h = ts[0]->h;
+    const bool async = ts[0]->async;
     for (int i = 0; i < k; ++i) {
         trl_trainer* t = ts[i];
         if (!t->own_stream) {
@@ -1531,6 +1597,7 @@ static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const 
         return rc;
     };
     auto hand_over = [&](int, trl_trainer* t) {
+        if (comm) return add_gathered_on(t, t->own_stream);
         if (h->train_slots) enqueue_add_slot(t, t->own_stream);
         else enqueue_add(t, h->B.tuples, h->B.tuple_flags, h->B.tuple_count, 0, h->B.tuple_cap, nullptr, t->own_stream, h->B.tuple_env);
         return 0;
@@ -1556,9 +1623,19 @@ static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const 
         }
         if (rc) break;
         if (phase != last_phase) { if ((rc = trl_set_terrain_lerp(h, phase))) break; last_phase = phase; }
+        if (async) {
+            for (int i = 0; i < k && rc == 0; ++i) rc = async_turnover(ts[i], iters_per_update);
+            if (rc || (rc = trl_update(h, time_step)) || (rc = trl_gather_tuples(h, block_rows))) break;
+            for (int i = 0; i < k; ++i) { ts[i]->job_pending = true; pos[i] += iters[i]; }
+            continue;
+        }
         if ((rc = trl_update(h, time_step))) break;
+        if (comm && (rc = trl_gather_tuples(h, block_rows))) break;
         if (!paced) {
-            rc = branch([&](int i, trl_trainer* t) { hand_over(i, t); return train_on(t, iters_per_update, t->own_stream); });
+            rc = branch([&](int i, trl_trainer* t) {
+                const int r = hand_over(i, t);
+                return r ? r : train_on(t, iters_per_update, t->own_stream);
+            });
         } else {
             rc = branch(hand_over);
             if (rc == 0 && (rc = read_counters()) == 0) {
@@ -1571,10 +1648,18 @@ static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const 
                 rc = branch([&](int i, trl_trainer* t) { return iters[i] > 0 ? train_on(t, iters[i], t->own_stream) : 0; });
             }
         }
-        cudaMemsetAsync(h->B.tuple_count, 0, 4, h->stream);      // cScenarioExp::ResetTupleBuffer, once every trainer has taken its rows
+        if (!comm) cudaMemsetAsync(h->B.tuple_count, 0, 4, h->stream);      // cScenarioExp::ResetTupleBuffer, once every trainer has taken its rows
         for (int i = 0; i < k; ++i) pos[i] += iters[i];
         const cudaError_t e = cudaGetLastError();
         if (rc == 0 && e != cudaSuccess) rc = trl_fail(std::string(who) + ": " + cudaGetErrorString(e));
+    }
+    if (async && rc == 0) {
+        // the trainer jobs of the last update, and the end of the stream of work: the caller's trl_sync must cover the trainers too
+        for (int i = 0; i < k && rc == 0; ++i) {
+            trl_trainer* t = ts[i];
+            if ((rc = async_turnover(t, iters_per_update))) break;
+            if (t->trained_pending) { cudaStreamWaitEvent(h->stream, t->ev_trained, 0); t->trained_pending = false; }
+        }
     }
     cudaEventDestroy(fork);
     if (hc) cudaFreeHost(hc);
@@ -1582,7 +1667,7 @@ static int run_slots_impl(const char* who, trl_trainer* const* ts, int k, const 
 }
 
 // what both entries refuse, with the handle unchanged
-static int check_slot_trainers(const char* who, trl_trainer* const* ts, int k) {
+static int check_slot_trainers(const char* who, trl_trainer* const* ts, int k, bool allow_async = false) {
     const std::string w(who);
     if (!ts || k < 1) return trl_fail(w + ": need at least one trainer");
     for (int i = 0; i < k; ++i) {
@@ -1590,8 +1675,26 @@ static int check_slot_trainers(const char* who, trl_trainer* const* ts, int k) {
         if (ts[i]->h != ts[0]->h) return trl_fail(w + ": the trainers belong to different handles");
         for (int j = 0; j < i; ++j)
             if (ts[j] == ts[i]) return trl_fail(w + ": trainer " + std::to_string(i) + " is listed twice");
-        if (ts[i]->async) return trl_fail(w + ": asynchronous trainers are not run in lock-step");
+        if (ts[i]->async && !allow_async) return trl_fail(w + ": asynchronous trainers are not run in lock-step");
     }
+    return 0;
+}
+
+// the per-trainer schedules' arguments (trl_train_run_slots_sched and trl_train_run_slots_comm)
+static int check_sched_args(const char* who, int k, const double* sp, int iters_per_update, int tuple_buffer_size) {
+    if (iters_per_update < 0) return trl_fail(std::string(who) + ": iters_per_update must be positive, or 0 for one iteration per tuple_buffer_size tuples");
+    if (iters_per_update == 0 && tuple_buffer_size < 1) return trl_fail(std::string(who) + ": tuple_buffer_size must be positive when the trainers are paced by tuples");
+    // one terrain blend per update for the whole handle: every trainer must be at the same curriculum phase at every update
+    bool all_off = true, same = true;
+    for (int i = 0; i < k; ++i) {
+        all_off = all_off && sp[9 * i + 8] < 1;
+        same = same && sp[9 * i + 8] == sp[8];
+    }
+    if (iters_per_update == 0 && !all_off)
+        return trl_fail(std::string(who) + ": trainers paced by tuples reach different curriculum phases (the handle has one terrain blend): "
+                        "every trainer_curriculum_iters must be < 1");
+    if (!all_off && !same)
+        return trl_fail(std::string(who) + ": the schedules differ in trainer_curriculum_iters (the handle has one terrain blend per update)");
     return 0;
 }
 
@@ -1610,21 +1713,57 @@ int trl_train_run_slots_sched(trl_trainer* const* ts, int k, const double* sp, i
     const char* who = "trl_train_run_slots_sched";
     if (check_slot_trainers(who, ts, k)) return 1;
     if (!sp) return trl_fail(std::string(who) + ": no schedules");
-    if (iters_per_update < 0) return trl_fail(std::string(who) + ": iters_per_update must be positive, or 0 for one iteration per tuple_buffer_size tuples");
-    if (iters_per_update == 0 && tuple_buffer_size < 1) return trl_fail(std::string(who) + ": tuple_buffer_size must be positive when the trainers are paced by tuples");
     if (ts[0]->h->comm) return trl_fail(std::string(who) + ": the handle has a communicator (multi-GPU training runs through trl_train_run)");
-    // one terrain blend per update for the whole handle: every trainer must be at the same curriculum phase at every update
-    bool all_off = true, same = true;
-    for (int i = 0; i < k; ++i) {
-        all_off = all_off && sp[9 * i + 8] < 1;
-        same = same && sp[9 * i + 8] == sp[8];
-    }
-    if (iters_per_update == 0 && !all_off)
-        return trl_fail(std::string(who) + ": trainers paced by tuples reach different curriculum phases (the handle has one terrain blend): "
-                        "every trainer_curriculum_iters must be < 1");
-    if (!all_off && !same)
-        return trl_fail(std::string(who) + ": the schedules differ in trainer_curriculum_iters (the handle has one terrain blend per update)");
+    if (check_sched_args(who, k, sp, iters_per_update, tuple_buffer_size)) return 1;
     return run_slots_impl(who, ts, k, sp, true, num_updates, iters_per_update, tuple_buffer_size, time_step);
+}
+
+// trl_train_run_slots_sched over the tuple exchange of a communicator: every rank's slot-p rows reach every rank's trainer p
+int trl_train_run_slots_comm(trl_trainer* const* ts, int k, const double* sp, int num_updates, int iters_per_update, int tuple_buffer_size,
+                             int block_rows, double time_step) {
+    const char* who = "trl_train_run_slots_comm";
+    const std::string w(who);
+    // the only refusals made alone: without a live first trainer and its handle's communicator there is no rank to agree with
+    if (!ts || k < 1) return trl_fail(w + ": need at least one trainer");
+    TRL_TRAINER_LIVE(ts[0]);
+    trl_handle* h = ts[0]->h;
+    if (!h->comm) return trl_fail(w + ": the handle has no communicator (trl_comm_init first; trl_train_run_slots_sched trains without one)");
+    // every other check is made here and then shared: all ranks take part in the one reduction below and refuse together
+    auto local_check = [&]() -> int {
+        if (check_slot_trainers(who, ts, k, true)) return 1;
+        if (!sp) return trl_fail(w + ": no schedules");
+        if (check_sched_args(who, k, sp, iters_per_update, tuple_buffer_size)) return 1;
+        int n_async = 0;
+        for (int i = 0; i < k; ++i) n_async += ts[i]->async ? 1 : 0;
+        if (n_async != 0 && n_async != k)
+            return trl_fail(w + ": " + std::to_string(n_async) + " of " + std::to_string(k) + " trainers are asynchronous (all or none)");
+        if (n_async && iters_per_update == 0)
+            return trl_fail(w + ": asynchronous training needs a fixed number of trainer iterations per update");
+        return 0;
+    };
+    const bool ok = local_check() == 0;
+    const std::string why = ok ? std::string() : std::string(trl_last_error());
+    // every rank must run the same call: the same slots in the same order under the same schedules, counts and modes
+    unsigned long long sig = trl::mix64((unsigned long long)k);
+    auto mix = [&](unsigned long long v) { sig = trl::mix64(sig + v); };
+    if (ok) {
+        for (int i = 0; i < k; ++i) {
+            mix((unsigned long long)ts[i]->slot);
+            mix(ts[i]->async ? 1ull : 0ull);
+            for (int j = 0; j < 9; ++j) { unsigned long long b; std::memcpy(&b, sp + 9 * i + j, 8); mix(b); }
+        }
+        mix((unsigned long long)(long long)iters_per_update);
+        mix((unsigned long long)(long long)(iters_per_update == 0 ? tuple_buffer_size : 0));
+        mix((unsigned long long)(long long)block_rows);
+    }
+    bool same = false, all_ok = false;
+    if (trl_comm_agree(h, sig, ok, &same, &all_ok)) return 1;
+    if (!ok) return trl_fail(why);
+    if (!all_ok) return trl_fail(w + ": another rank refused the call; every rank refuses it");
+    if (!same)
+        return trl_fail(w + ": the ranks differ in the call (listed slots, schedules, iters_per_update, tuple_buffer_size, block_rows or "
+                        "asynchronous trainers); every rank must train the same slots the same way");
+    return run_slots_impl(who, ts, k, sp, true, num_updates, iters_per_update, tuple_buffer_size, time_step, true, block_rows);
 }
 
 // c[9]: iter, actor_iter, stage, num, head, total, critic buffer, actor buffer, pending actor batch; l[2]: last losses

@@ -140,10 +140,14 @@ class Comm:
         self._ck(self.L.trl_trainer_replica_spread(trainer.h, C.byref(d)))
         return d.value
 
-    def EvalStats(self):
-        """cOptScenarioPoliEval::OutputResults' merge over all ranks (optimizer/scenarios/OptScenarioPoliEval.cpp:213-237)"""
+    def EvalStats(self, slot=None):
+        """cOptScenarioPoliEval::OutputResults' merge over all ranks (optimizer/scenarios/OptScenarioPoliEval.cpp:213-237);
+        slot: only the envs of that policy slot (trl_comm_eval_stats_slot, a learning curve per policy over all ranks)"""
         c = C.c_int64(0); e = C.c_int64(0); a = C.c_double(0); s = C.c_int64(0)
-        self._ck(self.L.trl_comm_eval_stats(self.sc.h, C.byref(c), C.byref(e), C.byref(a), C.byref(s)))
+        if slot is None:
+            self._ck(self.L.trl_comm_eval_stats(self.sc.h, C.byref(c), C.byref(e), C.byref(a), C.byref(s)))
+        else:
+            self._ck(self.L.trl_comm_eval_stats_slot(self.sc.h, int(slot), C.byref(c), C.byref(e), C.byref(a), C.byref(s)))
         return dict(cycles=c.value, episodes=e.value, avg_dist=a.value, steps=s.value)
 
     def TuplesDropped(self):

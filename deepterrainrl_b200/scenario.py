@@ -143,6 +143,7 @@ EXPORTS = [
     "trl_set_env_eval", "trl_env_eval", "trl_eval_stats_mode",
     "trl_load_body", "trl_set_env_body", "trl_env_body", "trl_eval_stats_body",
     "trl_load_body_range", "trl_load_physics_range", "trl_env_body_draws", "trl_env_physics_draws",
+    "trl_train_run_slots_comm", "trl_comm_eval_stats_slot",
 ]
 
 

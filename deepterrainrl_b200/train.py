@@ -157,7 +157,8 @@ class ScenarioTrainMACE:
         self.exp.OutputModel(path, mtime=int(time.time()))            # native writer behind the C ABI (csrc/model_io.h)
 
 
-def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step=1.0 / 30.0, tuple_buffer_size=32):
+def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step=1.0 / 30.0, tuple_buffer_size=32, comm=None,
+                    block_rows=1024):
     """cScenarioTrain::Run for several trainers of one exploration scenario: `num_updates` updates of the whole batch, each followed
     by every trainer's hand-over of its slot's tuples and its iterations, the trainers side by side on their own streams.
 
@@ -166,6 +167,11 @@ def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step
     call); None = each trainer paced as in ScenarioTrainMACE: one iteration per `tuple_buffer_size` fresh tuples of its slot, its
     schedule read at its own iteration count.  One schedule with a fixed count is trl_train_run_slots (applied handle-wide); every
     other call is trl_train_run_slots_sched.
+
+    comm: the scenario's parallel.Comm (multi-GPU, one process per GPU): trl_train_run_slots_comm, where every update's tuples of
+    all ranks go through ONE all-gather of up to `block_rows` rows per rank (the rest stays queued) and trainer p takes slot p's
+    rows of every rank.  Every rank must make the same call (same slots in the same order, schedules, counts; checked at the
+    start).  If every trainer is asynchronous (MACETrainer.SetAsync), each one's intake and iterations overlap the next update.
 
     A learning curve per slot, from evaluation envs of the same scenario (they run their slot's current net, exploration off, and
     feed no trainer)::
@@ -183,7 +189,7 @@ def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step
     L = trainers[0].L
     arr = (C.c_void_p * len(trainers))(*[t.h.value if t.h is not None else None for t in trainers])
     per_trainer = isinstance(schedule, (list, tuple))
-    if not per_trainer and iters_per_update is not None:
+    if comm is None and not per_trainer and iters_per_update is not None:
         sp = np.array([schedule.p[k] for k in TrainSchedule.KEYS], float)
         rc = L.trl_train_run_slots(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), int(iters_per_update),
                                    C.c_double(time_step))
@@ -194,8 +200,12 @@ def train_run_slots(trainers, schedule, num_updates, iters_per_update, time_step
         if iters_per_update is not None and int(iters_per_update) <= 0:
             raise ValueError("train_run_slots: iters_per_update must be positive, or None for tuple pacing")
         sp = np.array([[s.p[k] for k in TrainSchedule.KEYS] for s in scheds], float)
-        rc = L.trl_train_run_slots_sched(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates),
-                                         0 if iters_per_update is None else int(iters_per_update), int(tuple_buffer_size),
-                                         C.c_double(time_step))
+        ipu = 0 if iters_per_update is None else int(iters_per_update)
+        if comm is None:
+            rc = L.trl_train_run_slots_sched(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), ipu,
+                                             int(tuple_buffer_size), C.c_double(time_step))
+        else:
+            rc = L.trl_train_run_slots_comm(arr, len(trainers), sp.ctypes.data_as(C.c_void_p), int(num_updates), ipu,
+                                            int(tuple_buffer_size), int(block_rows), C.c_double(time_step))
     if rc != 0:
         raise RuntimeError(L.trl_last_error().decode())

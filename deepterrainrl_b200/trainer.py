@@ -114,6 +114,11 @@ class MACETrainer:
             self._ck(self.L.trl_trainer_add_device(self.h, C.c_void_p(r64[b:e].data_ptr()), C.c_void_p(f32[b:e].data_ptr()), e - b))
         self.scenario.Sync()                               # the tensors may be freed once the copies have run
 
+    def SetAsync(self, enable=True):
+        """Asynchronous training (trl_trainer_set_async): the intake and iterations run on their own stream beside the next update,
+        and the envs explore with a snapshot of the net refreshed between updates.  Needs a communicator on the scenario."""
+        self._ck(self.L.trl_trainer_set_async(self.h, 1 if enable else 0))
+
     def Train(self, iters=1):
         self._ck(self.L.trl_trainer_train(self.h, int(iters)))
 

@@ -334,7 +334,9 @@ int trl_train_run_timed(trl_trainer* t, const double* sp9, int num_updates, int 
 /* asynchronous training (the reference's asynchronous trainer: exploration keeps running on the net it has while the trainer works):
  * hand-over + trainer iterations run on their own stream beside the NEXT update inside trl_train_run / trl_train_run_timed; the
  * decision kernels read a snapshot of the net refreshed between updates (tuples of update u shape the policy from update u + 2 on).
- * Needs a communicator (a single rank will do) and a fixed iters_per_update. */
+ * Needs a communicator (a single rank will do) and a fixed iters_per_update.  A trainer of a handle with training slots may be made
+ * asynchronous only on a handle with a communicator (trl_train_run_slots_comm runs it): slot 0 then evaluates its snapshot through the
+ * handle's own net, a slot p >= 1 through its entry of the slot table; disabling binds the trainer's arrays again. */
 int trl_trainer_set_async(trl_trainer* t, int enable);
 int trl_trainer_counters(trl_trainer* t, int64_t* counters9, double* losses2);
 int trl_trainer_num_params(trl_trainer* t);
@@ -372,8 +374,9 @@ int trl_env_policy(trl_handle* h, int32_t* slots, int n);
  *   trl_trainer_create_slot  a trainer for slot 0 (the handle's own policy; trl_trainer_create(h, p) is the call with slot 0 and no
  *                        paths) or a training slot 1..7.  The starting net is the Caffe-HDF5 model + `_scale.txt` if both paths are
  *                        given, else a copy of the net slot 0 evaluates now.  Refused, with the handle unchanged, for a slot out of
- *                        range or with a trainer, a slot >= 1 on an evaluation handle, in the TRL_DECIDE_V1 build or on a handle
- *                        with a communicator, slot 0 on a handle with trl_load_policy slots, and a model of another topology.
+ *                        range or with a trainer, a slot >= 1 on an evaluation handle or in the TRL_DECIDE_V1 build, slot 0 on a
+ *                        handle with trl_load_policy slots, and a model of another topology.  On a handle with a communicator the
+ *                        trainers run through trl_train_run_slots_comm.
  *                        trl_trainer_destroy of a slot trainer leaves its trained net in the slot.
  *   trl_train_run_slots  the trl_train_run loop for k trainers of one handle in lock-step (iters_per_update > 0 each per update,
  *                        one exploration setting and curriculum blend per update, annealed from 0 in every call).  Refused for
@@ -385,14 +388,33 @@ int trl_env_policy(trl_handle* h, int32_t* slots, int n);
  *                        start of the update, one iteration per tuple_buffer_size fresh tuples of its slot, the remainder carried.
  *                        The handle keeps one terrain blend per update: refused unless every schedule has the same
  *                        trainer_curriculum_iters or all have it < 1 (paced: all < 1).  Also refused for whatever
- *                        trl_train_run_slots refuses, iters_per_update < 0 and, paced, tuple_buffer_size < 1.
+ *                        trl_train_run_slots refuses, iters_per_update < 0 and, paced, tuple_buffer_size < 1.  Both entries
+ *                        refuse a handle with a communicator and asynchronous trainers.
+ *   trl_train_run_slots_comm  the trl_train_run_slots_sched loop over N GPUs: per update the schedules, trl_update, ONE
+ *                        trl_gather_tuples(h, block_rows), then each trainer's slot-filtered trl_trainer_add_gathered and its
+ *                        iterations on its own stream, and the join.  Every rank sees the same blocks, so the counters and the
+ *                        replicas agree without a further collective, lock-step or paced (iters_per_update == 0, as
+ *                        trl_train_run_slots_sched paces); rows beyond block_rows stay queued.  With a single-rank
+ *                        communicator and block_rows >= the tuples of an update it computes, bit for bit, what
+ *                        trl_train_run_slots_sched computes on a handle without one.  If every listed trainer is
+ *                        asynchronous (trl_trainer_set_async), each one's intake and iterations overlap the next update as in
+ *                        trl_train_run: tuples of update u shape slot p's policy from update u + 2 on.  Every rank must make the same
+ *                        call: at its start the ranks compare the listed slots in order, the schedules, iters_per_update,
+ *                        tuple_buffer_size, block_rows and the asynchronous flags (one small all-reduce), and on a mismatch every
+ *                        rank refuses with nothing run.  Also refused: a mix of asynchronous and synchronous trainers,
+ *                        asynchronous trainers paced by tuples, and whatever trl_train_run_slots_sched refuses (its curriculum rule
+ *                        included); a rank that refuses one of these takes part in the same reduction, so every rank refuses
+ *                        together.  Refused by the calling rank alone: no trainer, a destroyed first trainer, no communicator.
  * Once a handle has a training slot: trl_trainer_add_from_scene hands a trainer only its slot's tuples and leaves the block to the
  * others (trl_reset_tuples clears it); trl_set_env_policy is refused while the block holds tuples and resets the envs it moves, so
- * every tuple belongs to the slot that chose its action; trl_train_run / trl_train_run_timed / trl_trainer_set_async are refused. */
+ * every tuple belongs to the slot that chose its action; trl_train_run / trl_train_run_timed are refused, and trl_trainer_set_async
+ * without a communicator. */
 trl_trainer* trl_trainer_create_slot(trl_handle* h, int slot, const double* params10, const char* h5_path, const char* scale_json_path);
 int trl_train_run_slots(trl_trainer* const* ts, int k, const double* sp9, int num_updates, int iters_per_update, double time_step);
 int trl_train_run_slots_sched(trl_trainer* const* ts, int k, const double* sp9k, int num_updates, int iters_per_update, int tuple_buffer_size,
                               double time_step);
+int trl_train_run_slots_comm(trl_trainer* const* ts, int k, const double* sp9k, int num_updates, int iters_per_update, int tuple_buffer_size,
+                             int block_rows, double time_step);
 
 /* number of tuples the engine could not record because the tuple block was full (cScenarioExp's ring overwrites, scenarios/
  * ScenarioExp.cpp:296-301; a batch block refuses instead and counts).  trl_num_tuples / trl_get_tuples* return
@@ -408,7 +430,9 @@ int trl_tuples_dropped(trl_handle* h, int64_t* out);
  *                          a device pack kernel (f32 rows like cMACETrainer's replay memory, learning/MACETrainer.cpp:515-539, flags,
  *                          global env ids, count header) + ONE all-gather of a fixed-capacity block per rank.  No host
  *                          synchronisation; rows beyond block_rows stay queued in the tuple block for the next call.
- *   trl_trainer_add_gathered   AddTuples of all gathered blocks (rank order, env order inside a rank) into the attached trainer
+ *   trl_trainer_add_gathered   AddTuples of all gathered blocks (rank order, env order inside a rank) into the attached trainer;
+ *                          in a handle with training slots, only the rows of the trainer's slot (flag bits 24..26), the others
+ *                          taking no replay slot
  *   trl_trainer_broadcast  cNeuralNetLearner::SyncNet across ranks (learning/NeuralNetLearner.cpp:85-89): weights + offset/scale
  *                          (and the trainer's target net / momentum history) from `root` to every rank
  *   trl_comm_eval_stats    cOptScenarioPoliEval::OutputResults' merge of the per-thread results
@@ -431,7 +455,10 @@ int trl_comm_info(trl_handle* h, int* rank, int* world, int* block_rows);
 int trl_comm_set_env_offset(trl_handle* h, int64_t env_offset);
 int trl_gather_tuples(trl_handle* h, int block_rows);
 /* gathered blocks as device memory: world blocks of block_bytes; block = {i32 count, i32 queued, i32 rank, i32 block_rows,
- * u32 flags[block_rows], i32 env[block_rows], f32 rows[block_rows][1+S+A+S]}.  Ordered on the handle's stream. */
+ * u32 flags[block_rows], i32 env[block_rows], f32 rows[block_rows][1+S+A+S]}.  Ordered on the handle's stream.  A row's flags are
+ * the tuple's flags (low bits) with bit 31 set if it fails cNeuralNetTrainer::CheckTuple and, in a handle with training slots,
+ * bits 24..26 holding the policy slot of the env that recorded it (zero in a handle without training slots).  Every trainer
+ * intake clears bits 24..31: a replay memory stores the tuple's own flags. */
 int trl_gathered_blocks(trl_handle* h, const void** dev_blocks, size_t* block_bytes, int* block_rows, int* row_width);
 /* host copy for tests / a CPU-side trainer: counts[world]; rows/flags/env may be NULL; cap in rows; synchronises */
 int trl_gathered_fetch(trl_handle* h, int32_t* counts, float* rows, uint32_t* flags, int32_t* env, int cap, int* n_total);
@@ -441,6 +468,8 @@ int trl_trainer_add_gathered(trl_trainer* t);
 int trl_trainer_broadcast(trl_trainer* t, int root);
 int trl_comm_broadcast_weights(trl_handle* h, int root);                       /* same for a handle without a trainer (eval ranks) */
 int trl_comm_eval_stats(trl_handle* h, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps);
+/* the same over the envs of one policy slot: trl_eval_stats_slot of every rank, summed (a learning curve per policy over all ranks) */
+int trl_comm_eval_stats_slot(trl_handle* h, int slot, int64_t* cycles, int64_t* episodes, double* avg_dist, int64_t* env_steps);
 /* max - min over ranks of every trainer parameter (replica drift check), via two all-reduces of +/-theta maxima; synchronises */
 int trl_trainer_replica_spread(trl_trainer* t, double* max_abs_diff);
 
